@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py -- MarlinKZG10/BLS12-381 commit+open at degree 2^20 (BASELINE.json configs[1]) on N B200s.
+"""bench.py -- MarlinKZG10/BLS12-381 commit+open at degree 2^20 (BASELINE.json configs[1]) on N H100s.
 
 A step = one KZG10 commit + one KZG10 open of one degree-2^20 polynomial (2^20+1 uniform Fr coefficients,
 hiding_bound=None, degree_bound=None: the protocol of bench-templates/src/lib.rs:69-138) = two G1 MSMs of
@@ -9,7 +9,10 @@ hiding_bound=None, degree_bound=None: the protocol of bench-templates/src/lib.rs
   e2e     the same through the C ABI with pinned HOST buffers (H2D of the coefficients inside the timed region,
           D2H of the two 96-byte points)
   roofline    dominant kernel (round 0 of the batched-affine pair rounds): algorithmic bytes (128 B per scalar-mult, SURVEY.md 8d) over the
-              average launch duration from CUDA events on the launching stream; peak = MEASURED_PEAKS.json hbm_gbs
+              average launch duration from CUDA events on the launching stream; peak = MEASURED_PEAKS.json hbm_gbs, else the
+              H100 SXM data sheet's 3.35 TB/s
+  --dump-outputs DIR  after the timed steps, writes the last step's commitment and witness (device-resident path) as float64
+              .npy files of 32-bit limbs; inputs are seeded, so two builds can be compared output for output
   cpu_baseline  the CPU oracle port (oracle/, OpenMP over Pippenger windows) timed on this box's host cores
   --impl reference   times that CPU path alone (the reference's Rust cannot be built here: no cargo/rustc)
 
@@ -44,7 +47,12 @@ def parse():
     ap.add_argument("--no-sharded", action="store_true", help="skip the sharded MSM / cfg5 / NTT sub-record")
     ap.add_argument("--sharded-log-n", type=int, default=22)
     ap.add_argument("--cfg5-polys", type=int, default=64)
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's commitment and witness to DIR/<name>.npy (float64 32-bit limbs)")
+    args = ap.parse_args()
+    if args.dump_outputs and args.impl != "pcgpu":
+        ap.error("--dump-outputs writes what the pcgpu path computed; it does not apply to --impl reference")
+    return args
 
 
 def measured_peaks():
@@ -52,11 +60,11 @@ def measured_peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons DURING the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,"
          "timestamp")
@@ -224,7 +232,7 @@ def main():
         dist = SingleDist()
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
-    eng = pc.Engine(local_rank)  # raises without the CUDA library / an sm_100 device
+    eng = pc.Engine(local_rank)  # raises without the CUDA library / an sm_90 device
     cid = pc.CURVES[CURVE]
     n = (1 << log_deg) + 1
 
@@ -266,7 +274,7 @@ def main():
         e0.record()
         torch.cuda.synchronize()
         t0 = time.perf_counter()
-        fn(k)
+        out = fn(k)
         torch.cuda.synchronize()
         wall_ms = (time.perf_counter() - t0) * 1e3
         e1.record()
@@ -276,18 +284,18 @@ def main():
             t = torch.tensor([ms], device="cuda")
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
             ms = float(t.item())
-        return ms
+        return ms, out
 
     sampler = ClockSampler(local_rank)
     sampler.start()                      # started before the warm-up so nvidia-smi is already streaming samples
     run_dev(max(warmup, 3))
     sampler.mark()
     l0 = eng.launch_count()
-    ms_dev = timed(run_dev, steps)
+    ms_dev, dev_out = timed(run_dev, steps)
     launches = eng.launch_count() - l0
     clocks = sampler.stop()
     run_host(max(warmup, 3))
-    ms_host = timed(run_host, steps)
+    ms_host, _ = timed(run_host, steps)
     # single-call latency (one polynomial per call: what a serial Rust caller of commit-then-open sees)
     eng.kzg_commit_open(srs, dev_polys[0].data_ptr(), z, n=n, flags=pc.DEVICE_PTRS)
     torch.cuda.synchronize()
@@ -322,6 +330,8 @@ def main():
         if world > 1:
             dist.destroy_process_group()
         return
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, *dev_out)
     polys = steps * world
     value = polys / (ms_dev / 1e3)
     e2e = polys / (ms_host / 1e3)
@@ -338,7 +348,6 @@ def main():
     dom_ms = pair0_ms / pair0_cnt if pair0_cnt else (acc_ms / max(acc_cnt, 1))
     dom_name = "run_kernel_occ<MsmAffinePairBody<Bls12381, true>>" if pair0_cnt else "run_persistent_kernel<MsmAccumulateBody<Bls12381>>"
     achieved = (n * ALGO_BYTES_PER_SCALAR_MULT / 1e9) / (dom_ms / 1e3) if dom_ms else None
-    traffic, traffic_src = ncu_traffic(log_deg)
     line = {
         "metric": "MarlinKZG10/BLS12-381 commit+open polys/s at deg 2^20", "value": value, "unit": "polys/s",
         "n_gpus": world, "steps": steps, "warmup": warmup, "ms_per_step": ms_dev / steps, "higher_is_better": True,
@@ -347,7 +356,7 @@ def main():
         "config": {"workload": workload, "parallelism": f"poly-sharded x{world}, SRS replicated; one batch call per rank, 2 polynomials "
                    "(4 MSM pipelines) in flight inside the library",
                    "l2": "per-step working set (window-folded SRS tables 1.5 GB gather + 34 MB coefficients, rotating "
-                         "polynomials) exceeds the 126 MB L2; no explicit flush"},
+                         "polynomials) exceeds the 50 MB L2; no explicit flush"},
         "msm_scalar_mults_per_s": 2 * n * polys / (ms_dev / 1e3),
         "stage_ms_per_step": stage_ms,
         "single_call_ms_per_step": ms_single_call,
@@ -356,7 +365,7 @@ def main():
         "gpu_launches": launches,
         "clocks": clocks,
         "roofline": {"bound": "hbm", "kernel": dom_name, "achieved": achieved, "peak": peak,
-                     "unit": "GB/s", "frac": (achieved / peak) if achieved else None, "traffic": traffic, "traffic_source": traffic_src,
+                     "unit": "GB/s", "frac": (achieved / peak) if achieved else None,
                      "peak_source": peak_src, "launch_ms": dom_ms,
                      "compute_roofline": {"bound": "int32 multiply pipe (IMAD.WIDE.U32)", "peak_wide_mul_per_s": imad_peak,
                                           "achieved_wide_mul_per_s": wide_per_msm / (msm_kernel_ms / 1e3) if msm_kernel_ms else None,
@@ -402,17 +411,15 @@ class SingleDist:
         out.copy_(inp)
 
 
-def ncu_traffic(log_deg):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one launch of the dominant kernel, from the committed ncu --set full
-    capture of THIS code (profiles/r02_ncu_pair0_traffic.json, written by tools/ncu_traffic.py from the capture's raw page)"""
-    try:
-        with open(os.path.join(ROOT, "profiles", "r02_ncu_pair0_traffic.json")) as f:
-            d = json.load(f)
-        if int(d.get("log_deg", -1)) == log_deg:
-            return int(d["dram_bytes_read"]) + int(d["dram_bytes_write"]), d.get("source")
-    except Exception:
-        pass
-    return None, None
+def dump_outputs(out_dir, comm, comm_inf, w, w_inf):
+    """The last timed step's results as a caller of pcgpu_kzg_commit_open_batch receives them: affine x || y of the
+    commitment and of the witness (uint64 limbs, split into 32-bit limbs so float64 holds them exactly) and their
+    identity flags.  A few hundred bytes in all."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, xy, inf in (("commitment", comm, comm_inf), ("witness", w, w_inf)):
+        np.save(os.path.join(out_dir, f"{name}_xy.npy"), np.ascontiguousarray(xy[-1]).view(np.uint32).astype(np.float64))
+        np.save(os.path.join(out_dir, f"{name}_is_identity.npy"), np.asarray(inf[-1:], dtype=np.float64))
 
 
 def sharded_record(args, eng, pc, params, sharded, dist, dev, rank, world, cid):

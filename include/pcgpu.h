@@ -1,8 +1,8 @@
 /*
- * pcgpu.h -- C ABI of the B200-native polynomial-commitment compute engine.
+ * pcgpu.h -- C ABI of the H100-native polynomial-commitment compute engine.
  *
- * This is the drop-in boundary for the hot path of arkworks-rs/poly-commit (reference mounted at
- * /root/reference; all file:line citations below are relative to it).  The reference has no FFI of
+ * This is the drop-in boundary for the hot path of arkworks-rs/poly-commit (reference @ a05ec99;
+ * all file:line citations below are relative to its root).  The reference has no FFI of
  * its own: the path sits behind Rust trait methods of un-vendored crates (ark-ec / ark-poly 0.5.0).
  * Each entry point therefore names the Rust call it replaces; INTEGRATION.md shows the Rust-side
  * `extern "C"` declarations and the patched call sites.
@@ -19,7 +19,7 @@
  *     0 = success, negative = error (pcgpu_strerror).
  *   - Thread safety: calls on one pcgpu_ctx are serialised by an internal mutex; use one context
  *     per host thread for concurrency (hyrax/mod.rs:233-242 calls msm from a Rayon par_iter).
- *   - There is no CPU fallback: every entry point fails with PCGPU_E_CUDA when no sm_100 device
+ *   - There is no CPU fallback: every entry point fails with PCGPU_E_CUDA when no sm_90 device
  *     is usable.
  */
 #ifndef PCGPU_H

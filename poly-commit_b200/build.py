@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
-"""Builds poly-commit_b200/libpcgpu.so: nvcc, sm_100a only, one translation unit per (curve, kernel group) in parallel.
-No GPU is needed to build (nvcc cross-compiles).  Re-builds only when a source is newer than the library."""
+"""Builds poly-commit_b200/libpcgpu.so: nvcc, sm_90a (H100) only, one translation unit per (curve, kernel group) in parallel.
+No GPU is needed to build (nvcc cross-compiles).  Re-builds only when a source or this script (architecture, flags) is newer than the library."""
 import concurrent.futures
 import glob
 import os
@@ -16,12 +16,13 @@ CURVES = ["Bls12381", "Bn254", "Pallas"]
 GROUPS = [6, 8, 9, 5, 2, 3, 1, 4]   # inst_unit.cu groups, heaviest first (see the list at the top of that file)
 # heaviest first so the thread pool keeps every core busy to the end
 UNITS = [("inst_unit", c, g) for g in GROUPS for c in CURVES] + [("api", None, None)]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
 
 
 def _newest_source():
     srcs = glob.glob(os.path.join(CSRC, "*.cu")) + glob.glob(os.path.join(CSRC, "*.cuh")) + \
-        glob.glob(os.path.join(CSRC, "*.hpp")) + [os.path.join(HERE, "..", "include", "pcgpu.h")]
+        glob.glob(os.path.join(CSRC, "*.hpp")) + [os.path.join(HERE, "..", "include", "pcgpu.h"), os.path.abspath(__file__)]
     return max(os.path.getmtime(s) for s in srcs)
 
 
@@ -53,7 +54,7 @@ def build(force=False, verbose=False, extra=()):
             raise RuntimeError(f"nvcc failed on {unit}.cu")
         objs.append(out)
     # link next to the target and rename: a reader (or a snapshot of the tree) never sees a half-written library
-    subprocess.check_call(["nvcc", "-shared", "-o", LIB + ".tmp"] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"])
+    subprocess.check_call(["nvcc", "-shared", "-o", LIB + ".tmp"] + objs + ARCH)
     os.replace(LIB + ".tmp", LIB)
     return LIB
 

@@ -21,7 +21,7 @@ PCGPU_INSTANTIATE(Pallas, extern)
 extern "C" const char *pcgpu_strerror(int code) {
   switch (code) {
     case PCGPU_OK: return "ok";
-    case PCGPU_E_CUDA: return "CUDA failure or no usable sm_100 device";
+    case PCGPU_E_CUDA: return "CUDA failure or no usable sm_90 device";
     case PCGPU_E_OOM: return "device memory allocation failed";
     case PCGPU_E_BADARG: return "bad argument";
     case PCGPU_E_LEN: return "length out of range (base_offset + n exceeds the registered bases, or the input is longer than the transform / slice)";
@@ -43,10 +43,10 @@ extern "C" int pcgpu_init(int device, pcgpu_ctx **out) {
   if (cudaGetDeviceCount(&count) != cudaSuccess || device < 0 || device >= count) return PCGPU_E_CUDA;
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return PCGPU_E_CUDA;
-  if (prop.major != 10) return PCGPU_E_CUDA;  // built for sm_100a only; no other code path exists
+  if (prop.major != 9 || prop.minor != 0) return PCGPU_E_CUDA;  // built for sm_90a only; no other code path exists
   if (cudaSetDevice(device) != cudaSuccess) return PCGPU_E_CUDA;
   // L2 fetch granularity hint: the table gathers of the pair rounds read ONE 64-byte half record (x in pass 1, y in pass 2)
-  // per access; at the default granularity every such miss moves a whole 128-byte line from DRAM (ncu: 680 B read per slot).
+  // per access; at the default granularity every such miss moves a whole 128-byte line from DRAM.
   if (const char *e = getenv("PCGPU_L2_FETCH_GRANULARITY")) {
     int v = atoi(e);
     if (v == 32 || v == 64 || v == 128) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)v);
@@ -701,7 +701,7 @@ extern "C" int pcgpu_kzg_commit_open(pcgpu_ctx *ctx, const pcgpu_srs *powers_of_
   });
 }
 
-enum { PCGPU_COMMIT_OPEN_WAYS = 2, PCGPU_COMMIT_OPEN_MAX_WAYS = 4, PCGPU_BATCH_PAIR_TDIV = 2 };   // half-wave pair kernels in batch mode: +2.5 % (profiles/r02_l2_tdiv_ab.txt)   // polynomials in flight (two MSM pipelines each)
+enum { PCGPU_COMMIT_OPEN_WAYS = 2, PCGPU_COMMIT_OPEN_MAX_WAYS = 4, PCGPU_BATCH_PAIR_TDIV = 2 };   // polynomials in flight (two MSM pipelines each); half-wave pair kernels in batch mode
 
 extern "C" int pcgpu_kzg_commit_open_batch(pcgpu_ctx *ctx, const pcgpu_srs *powers_of_g, const void *const *coeffs, const size_t *n,
                                            size_t count, const void *z, uint32_t flags, void *out_comm_xy, uint8_t *out_comm_inf,

@@ -1,4 +1,4 @@
-// Prime-field arithmetic for sm_100a: N x 32-bit limbs held in registers, Montgomery form
+// Prime-field arithmetic for sm_90a: N x 32-bit limbs held in registers, Montgomery form
 // with R = 2^(32 N) (identical to ark-ff's 2^(64 N/2), so the byte image of an element equals
 // ark-ff's Fp<MontBackend, N/2>; SURVEY.md section 8b "Data conventions").
 //

@@ -443,8 +443,8 @@ inline int fr_div_linear(const uint32_t *p, size_t n, const uint32_t *z, uint32_
     if (c <= DIV_F || levels == DIV_MAX_LEVELS) break;
   }
   int rc;
-  // one pass up to 2^21 coefficients (0.08 / 0.15 ms at 2^16 / 2^20 against 0.17 / 0.21 ms for the level tree below); beyond
-  // that the level tree's fewer products per coefficient win (0.35 against 0.41 ms at 2^22); PCGPU_DIV_MODE = tile | tree forces one
+  // one pass up to 2^21 coefficients; beyond that the level tree's fewer products per coefficient win;
+  // PCGPU_DIV_MODE = tile | tree forces one
   if (div_one_pass(n)) {
     // one pass: powers (one small launch), control words cleared, tiles chained by a decoupled look-back
     const uint32_t ntiles = (uint32_t)((n + DIVT_TILE - 1) / DIVT_TILE);
@@ -453,8 +453,8 @@ inline int fr_div_linear(const uint32_t *p, size_t n, const uint32_t *z, uint32_
     if ((rc = rt::launch<64>(DivTilePowersBody<R>{z, pw}, DIVT_POW_COUNT, st))) return rc;
     return rt::launch_blocks<DIVT_THREADS>(DivTileBody<R>{p, n, z, pw, q, rem, ctl, aggp, incp, ntiles}, ntiles, divt_smem_bytes(), st);
   }
-  // (a three-launch variant with ONE block scanning all chunk carries was measured slower: 0.99 ms vs 0.36 ms at 2^22 -- 128
-  // dependent products per thread twice over; the level tree below keeps every chain at DIV_F = 32)
+  // (a three-launch variant with ONE block scanning all chunk carries has 128 dependent products per thread twice over;
+  // the level tree below keeps every chain at DIV_F = 32)
   if (getenv("PCGPU_DIV_BLOCK_SCAN") && cnt[0] <= (size_t)DIV_SCAN_BLOCK * 4096) {
     if ((rc = rt::launch<128>(DivChunkLocalBody<R>{p, n, z, local[0]}, cnt[0], st))) return rc;
     if ((rc = rt::launch_blocks<DIV_SCAN_BLOCK>(DivBlockScanBody<R>{local[0], cnt[0], z, carry[0], rem}, 1, (16 * DIV_SCAN_BLOCK + 32) * 4, st))) return rc;

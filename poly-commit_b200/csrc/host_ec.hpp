@@ -1,10 +1,9 @@
 // Host-side finishing arithmetic: the last O(c) group operations of an MSM and the projective ->
 // affine conversion, on 64-bit limbs.
 //
-// Why the host: a lone GPU thread retires one 381-bit Montgomery product per ~1 us (measured:
-// a Fermat inversion took 0.6 ms on the device), so any strictly serial chain -- the Horner
-// combination of the c bit-plane sums and the single field inversion -- is ~20x faster on a CPU
-// core.  The device does all O(n) work and hands back S*c points (3 KB for c = 16); this file adds
+// Why the host: a lone GPU thread retires one 381-bit Montgomery product far more slowly than a
+// CPU core, so any strictly serial chain -- the Horner combination of the c bit-plane sums and the
+// single field inversion -- is faster on the host.  The device does all O(n) work and hands back S*c points (3 KB for c = 16); this file adds
 // them up.  It mirrors what the reference itself does on the CPU after the MSM:
 // `commitment.into()` / `w.into_affine()` (kzg10/mod.rs:209, :281).  It is product code (always
 // executed, never a substitute for the kernels) and shares nothing with oracle/.

@@ -1,7 +1,7 @@
 // Host-side implementation templates behind the C ABI (include/pcgpu.h).  Host logic only: argument checks that mirror the
 // reference's error behaviour, staging of host buffers, stage timing, and curve dispatch.
 //
-// Compiled by nvcc for sm_100a into libpcgpu.so (the product).  The same file is also compiled by
+// Compiled by nvcc for sm_90a into libpcgpu.so (the product).  The same file is also compiled by
 // g++ with -DPCGPU_EMUL into tests/host_emul/libpcgpu_hostcheck.so, a unit-test harness that runs
 // the kernel bodies serially; the package never loads that library.
 #pragma once
@@ -121,8 +121,8 @@ static const int NSLOTS = 8;
 template <class C> static int ensure_pow2(pcgpu_ctx *ctx);
 
 // comb window bits: the widest window whose tables (n * W * 2^(c-1) points) fit the budget: PCGPU_COMB_MAX_GB if set, else
-// 40 % of the device memory that is free right now, at most 72 GB (cfg4 on a 180 GB B200: c = 16, 16 windows, 69 GB, built in
-// 1.8 s once per key; 13.1 ms per 2^11-row commit against 15.4 ms at the former 24 GB cap)
+// 40 % of the device memory that is free right now, at most 72 GB (wider windows mean fewer bucket additions per commit;
+// the table is built once per key)
 inline uint32_t comb_window_bits(size_t n, size_t point_bytes) {
   if (const char *e = getenv("PCGPU_COMB_C")) { int v = atoi(e); if (v >= 4 && v <= 16) return (uint32_t)v; }
   double cap = 24e9;
@@ -962,8 +962,7 @@ int ipa_round_lr_impl(pcgpu_ctx *ctx, pcgpu_ctx *sib, pcgpu_ipa *st, const void 
     return PCGPU_OK;
   }
   if (m <= 2 * SMALL_MAX_N && msm_small_enabled()) {
-    // rounds of <= 8192-term commitments (1.6 ms each through the bucket pipeline, whose fixed cost dominates at this size;
-    // 0.5 - 0.7 ms here): both commitments, each with its  + h' * <.,.>  term, in ONE launch; the inner products never leave HBM
+    // rounds of <= 8192-term commitments (the bucket pipeline's fixed cost dominates at this size): both commitments, each with its  + h' * <.,.>  term, in ONE launch; the inner products never leave HBM
     uint32_t *d_h = st->d_scr + 8 * (IP_THREADS + IP_THREADS / IP_BLOCK + 12);   // 3 slots, clear of d_ip / d_ch
     if ((rc = fr_inner_product<R>(cr, zl, m, d_ip, st->d_scr, s))) return rc;
     if ((rc = fr_inner_product<R>(cl, zr, m, d_ip + 8, st->d_scr, s))) return rc;
@@ -1489,7 +1488,10 @@ inline int measure_imad_peak_impl(pcgpu_ctx *ctx, double *ops_per_s) {
 #else
   rt::stream_t st = ctx->stream;
   int rc;
-  const size_t threads = 148 * 2048;   // full occupancy on B200
+  int dev = 0, sms = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+    return PCGPU_E_CUDA;
+  const size_t threads = (size_t)sms * 2048;   // full occupancy: 2048 resident threads per SM
   const uint32_t iters = 4096;
   if ((rc = ctx->stage.reserve(threads * 8 + 4096))) return rc;
   uint64_t *sink = ctx->stage.take<uint64_t>(threads);

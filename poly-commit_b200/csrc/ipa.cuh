@@ -89,7 +89,7 @@ struct G1FoldGlvBody {
       const bool n1 = (u1_nz[w] >> sh) & 1, n2 = (u2_nz[w] >> sh) & 1, s1 = (u1_sg[w] >> sh) & 1, s2 = (u2_sg[w] >> sh) & 1;
       if (!(n1 || n2)) continue;
       // the table point is SELECTED (register moves) and added at ONE call site: with an addition inlined per case the loop
-      // body outgrows the instruction cache (measured on the small-MSM kernel: -18 % from out-of-line additions alone)
+      // body outgrows the instruction cache
       Affine<C> a = p1;
       bool neg = s1;
       if (n1 && n2) { if (s1 == s2) a = ps; else a = pd; }      // +-(P1 + P2) / +-(P1 - P2): the sign is u1's

@@ -4,7 +4,7 @@
 // additions the inversion is shared: 3 multiplications per element plus ONE inversion per batch, i.e.
 // ~6.2 modular multiplications per addition instead of the 9.5 of the XYZZ mixed addition -- provided the
 // shared inversion is cheap.  It is: fp_inv_gcd runs on the ALU pipe, which idles while the integer-multiply
-// pipe saturates (ncu: fmaheavy 83 %, alu 16 %), so across warps the two overlap.
+// pipe saturates, so across warps the two overlap.
 //
 // Independent additions come from pairing neighbours inside every bucket: round r turns the cnt_b points of
 // bucket b into ceil(cnt_b / 2) points (an odd one out is copied).  Thread t of a round owns the output slots

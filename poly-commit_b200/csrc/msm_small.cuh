@@ -1,12 +1,12 @@
 // Small multi-scalar multiplications (n <= SMALL_MAX_N) in ONE launch.
 //
 // The bucket pipeline of msm.cuh is built for 2^16 .. 2^26 terms: a dozen launches, a counting sort and a host tail over
-// S * c bit planes cost ~1 ms however few points there are (profiles/r01_small_msm_probe.json: 1.3 ms at 2^10 on BLS12-381,
-// of which 0.49 ms is the host combining 26 windows x 10 planes).  The callers with few terms -- the late rounds of the IPA
+// S * c bit planes have a fixed cost however few points there are (at 2^10 on BLS12-381 the host alone combines 26 windows
+// x 10 planes).  The callers with few terms -- the late rounds of the IPA
 // halving loop (ipa_pc/mod.rs:665-711), the verifier-side combinations (hyrax/mod.rs:498-504, kzg10/mod.rs:322-373), cfg1's
 // degree-2^10 commitments (kzg10/mod.rs:175-178) -- run here instead:
 //   grid  = (#problems) x W x split blocks, W = ceil((bits + 2) / c) windows of c = 6 bits; a window's terms are divided
-//           among `split` blocks (1 below 512 terms, else 3: 129 blocks on the 148 SMs), each producing a partial U_w
+//           among `split` blocks (1 below 512 terms, else 3: 129 blocks, one wave on the 132 SMs of an H100), each producing a partial U_w
 //   block = 256 threads = 32 buckets (digit magnitudes 1..32) x 8 slices of the scalars
 //   1. digits: signed digits d in [-32, 31] by the offset trick: the base-2^c digits e_w of s + K, K = sum_w 2^(c-1) 2^(cw),
 //      give d_w = e_w - 2^(c-1) with sum_w d_w 2^(cw) = s -- every window is computed independently, no carry chain

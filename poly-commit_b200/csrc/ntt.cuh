@@ -148,7 +148,7 @@ template <class Body>
 inline int ntt_launch(const Body &b, size_t nblocks, size_t smem_bytes, rt::stream_t st) {
   const uint32_t M = 1u << b.m;
   // (only when the grid is large enough to fill the device with narrow blocks; a small grid is latency-bound and wants the
-  // wide block's parallel loads and stores: 2^16 = 256 x 256 runs 0.055 ms with 128 threads, 0.069 ms with 32)
+  // wide block's parallel loads and stores)
   if (nblocks < 4096) return rt::launch_blocks_occ<NTT_BLOCK, NTT_MIN_BLOCKS>(b, nblocks, smem_bytes, st);
   if (M <= 256) return rt::launch_blocks_occ<32, 16>(b, nblocks, smem_bytes, st);
   if (M <= 512) return rt::launch_blocks_occ<64, 8>(b, nblocks, smem_bytes, st);
@@ -244,8 +244,9 @@ inline int ntt_build_plan(NttPlan &p, int curve, uint32_t logn, int inverse, rt:
   p.curve = curve; p.logn = logn; p.inverse = inverse;
   ntt_split(logn, &p.m1, &p.m2);
   size_t n1h = (size_t)1 << (p.m1 ? p.m1 - 1 : 0), n2h = p.m2 ? (size_t)1 << (p.m2 - 1) : 1;
-  // step-2 twiddles w_N^e: up to N = 2^NTT_FULL_TABLE_MAX_LOG the whole table (32 MB at 2^20, L2-resident next to the vector: one
-  // load and ONE product per element of pass 1); beyond, hi[e >> 10] * lo[e & 1023] (two products)
+  // step-2 twiddles w_N^e: up to N = 2^NTT_FULL_TABLE_MAX_LOG the whole table (32 MB at 2^20: one load and ONE product per
+  // element of pass 1; with the 32 MB vector it does not fit a 50 MB L2, so the table is streamed from HBM once per pass);
+  // beyond, hi[e >> 10] * lo[e & 1023] (two products, both tables cache-resident)
   const bool full = p.m2 != 0 && logn <= NTT_FULL_TABLE_MAX_LOG;
   size_t nlo = full ? 0 : (size_t)1 << NTT_LO_BITS;
   size_t nhi = full ? (size_t)1 << logn : (logn > NTT_LO_BITS ? (size_t)1 << (logn - NTT_LO_BITS) : 1);

@@ -5,7 +5,7 @@
 // -DPCGPU_EMUL (tests/host_emul only -- a unit-test harness, never shipped, never loaded by the
 // package) the same bodies run in a serial loop and "device" memory is host memory, which lets the
 // limb schedules, digit recoding, bucket bookkeeping and scan logic be checked on a machine
-// without a GPU.  The product build (nvcc, sm_100a) contains no host execution path.
+// without a GPU.  The product build (nvcc, sm_90a) contains no host execution path.
 #pragma once
 #include <stddef.h>
 #include <stdint.h>

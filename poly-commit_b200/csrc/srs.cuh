@@ -5,7 +5,7 @@
 // Table group k holds 2^(c*k) * P_i (affine).  With all W groups present every Pippenger window
 // shares ONE bucket set (window w of scalar i adds group-w's copy of base i), so the MSM tail needs
 // no doublings and the bucket reduction shrinks from W*2^(c-1) to 2^(c-1) buckets.  Cost: W x the
-// SRS footprint (1.6 GB for 2^20 BLS12-381 bases at c = 16 -- small against 180 GB of HBM3e).
+// SRS footprint (1.6 GB for 2^20 BLS12-381 bases at c = 16 -- small against 80 GB of HBM3).
 #pragma once
 #include "ec.cuh"
 #include "msm.cuh"
@@ -19,7 +19,7 @@ inline uint32_t srs_precompute_window(size_t n) {
   if (const char *e = getenv("PCGPU_SRS_C")) { int v = atoi(e); if (v >= 8 && v <= 22) return (uint32_t)v; }   // tuning knob
   uint32_t lg = ilog2_floor(n ? n : 1);
   if (lg >= 18) return 17;   // 255 / 17 = 15 windows (load_scalar halves the scalar range, no 16th carry window): 6 % fewer
-                             // additions than c = 16 -- equal single-MSM latency, +5 % batch throughput (profiles/r02_bench_n1_*)
+                             // additions than c = 16
   if (lg >= 15) return 14;
   return 12;
 }

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with `-m gpu` on a B200): the CUDA library through its C ABI against the CPU oracle
+"""GPU parity tests (run with `-m gpu` on an H100): the CUDA library through its C ABI against the CPU oracle
 on the same seeded inputs -- bit-exact (all arithmetic is integer / finite field; tolerance = 0).
 
 Small and medium sizes compare directly against the oracle (definition-level MSM or its Pippenger); the
@@ -461,8 +461,7 @@ def test_concurrent_host_threads(eng, pc):
 
 def test_randomised_sweep(capsys):
     """A short run of tests/perf/fuzz_gpu.py (random shapes across the small-path / split / bucket-pipeline boundaries, scalar
-    mixtures, base offsets, the three division modes, NTT + inverse, hiding commits / opens), bit-exact against the C oracle;
-    profiles/r02_fuzz_gpu.log holds two 400-case runs."""
+    mixtures, base offsets, the three division modes, NTT + inverse, hiding commits / opens), bit-exact against the C oracle."""
     import importlib.util
     import os
     import sys

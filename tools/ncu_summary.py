@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """Per-kernel summary of an `ncu --set full` report exported with `ncu -i X.ncu-rep --page raw --csv`: one line per launch with
 duration, DRAM bytes and fraction of peak, pipe activity, occupancy, registers.
-    python tools/ncu_summary.py /tmp/raw.csv > profiles/rNN_ncu_<what>_summary.txt"""
+    python tools/ncu_summary.py perf_out/raw.csv > perf_out/ncu_<what>_summary.txt"""
 import csv
 import sys
 
