@@ -331,6 +331,26 @@ int pcgpu_measure_imad_peak(pcgpu_ctx *ctx, double *ops_per_s);
 /* Kernels launched by this library in the calling process so far (bench.py's gpu_launches). */
 uint64_t pcgpu_launch_count(void);
 int pcgpu_selftest_field(pcgpu_ctx *ctx, int curve, uint64_t seed, size_t n, uint64_t *mismatches);
+/* The path and geometry the context's most recent MSM took, each value recorded where the library decided it.  Writes
+ * min(len, PCGPU_GEOM_FIELDS) words: out[PCGPU_GEOM_PATH] is PCGPU_MSM_PATH_NONE (n = 0, or no MSM yet), _SMALL (one-launch
+ * kernel; out[PCGPU_GEOM_SPLIT] = blocks per window: 1, 3 or 6) or _BUCKETS (the bucket pipeline: window bits c, windows W,
+ * table groups G (1 = raw bases), batched-affine rounds R, the pair-round kernel's threads T and its divisor tdiv, the one
+ * resident wave of that kernel the round count was chosen against, entries = n * W, and the number of buckets reduced by
+ * the heavy-bucket kernel, or UINT64_MAX where the pipeline's tail did not report it).  Unused fields are 0. */
+enum {
+  PCGPU_GEOM_PATH = 0, PCGPU_GEOM_SPLIT = 1, PCGPU_GEOM_N = 2, PCGPU_GEOM_C = 3, PCGPU_GEOM_W = 4, PCGPU_GEOM_G = 5,
+  PCGPU_GEOM_R = 6, PCGPU_GEOM_T = 7, PCGPU_GEOM_TDIV = 8, PCGPU_GEOM_WAVE = 9, PCGPU_GEOM_ENTRIES = 10,
+  PCGPU_GEOM_HEAVY = 11, PCGPU_GEOM_FIELDS = 12
+};
+enum { PCGPU_MSM_PATH_NONE = 0, PCGPU_MSM_PATH_SMALL = 1, PCGPU_MSM_PATH_BUCKETS = 2 };
+int pcgpu_msm_last_geometry(pcgpu_ctx *ctx, uint64_t *out, size_t len);
+/* One field primitive applied elementwise on the device (the same code the kernels use), for testing the field layer
+ * against plain integers: which = 0 the base field Fq of `curve`, 1 its scalar field Fr.  a, b, out: host arrays of n
+ * elements, little-endian 32-bit limbs (Fq of BLS12-381: 12 limbs, every other field 8), Montgomery form.  op:
+ *   0 mont_mul(a, b)   1 mont_mul_ref(a, b) (plain 64-bit accumulate)   2 a + b   3 a - b   4 -a   5 a^-1 (Fermat)
+ *   6 mont_mul2(a, b, b, -a) (= 0)   7 mont_mul2(a, b, a + b, b - a)   8 a^-1 (binary GCD)   9 mont_sqr(a)
+ * Ops 6 and 7 fall back to two products on a field without mont_mul2; inverses of 0 are 0. */
+int pcgpu_diag_field_op(pcgpu_ctx *ctx, int curve, int which, int op, const void *a, const void *b, void *out, size_t n);
 
 #ifdef __cplusplus
 }

@@ -7,6 +7,9 @@ import numpy as np
 
 BLS12_381, BN254, PALLAS = 0, 1, 2
 CURVES = {"bls12_381": BLS12_381, "bn254": BN254, "pallas": PALLAS}
+# pcgpu_msm_last_geometry: field names in the header's PCGPU_GEOM_* order, and the PCGPU_MSM_PATH_* values
+GEOM_FIELDS = ("path", "split", "n", "c", "W", "G", "R", "T", "tdiv", "wave", "entries", "heavy")
+MSM_PATH_NONE, MSM_PATH_SMALL, MSM_PATH_BUCKETS = 0, 1, 2
 SCALARS_MONT, DEVICE_PTRS, SRS_PRECOMPUTE, NTT_INVERSE, SRS_COMB, WIRE_COMPRESSED, WIRE_NO_VALIDATE = 1, 2, 4, 8, 16, 32, 64
 E_INVALID = -8
 
@@ -81,6 +84,8 @@ def _load(path):
         "pcgpu_fr_row_mul": [_vp, ctypes.c_int, _vp, _vp, _sz, _sz, _vp, ctypes.c_uint32],
         "pcgpu_measure_imad_peak": [_vp, ctypes.POINTER(ctypes.c_double)],
         "pcgpu_selftest_field": [_vp, ctypes.c_int, ctypes.c_uint64, _sz, ctypes.POINTER(ctypes.c_uint64)],
+        "pcgpu_msm_last_geometry": [_vp, ctypes.POINTER(ctypes.c_uint64), _sz],
+        "pcgpu_diag_field_op": [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp, _sz],
         "pcgpu_ipa_begin": [_vp, ctypes.c_int, _vp, _sz, _vp, _sz, _vp, ctypes.c_uint32, ctypes.POINTER(_vp)],
         "pcgpu_ipa_round_lr": [_vp, _vp, _vp, _vp, _vp, _vp, _vp],
         "pcgpu_ipa_round_fold": [_vp, _vp, _vp, _vp],
@@ -279,6 +284,26 @@ class Engine:
         bad = ctypes.c_uint64()
         self._ck(self.lib.pcgpu_selftest_field(self.ctx, curve, seed, n, ctypes.byref(bad)))
         return bad.value
+
+    def msm_last_geometry(self):
+        """dict of the path and geometry the most recent MSM on this context took (pcgpu_msm_last_geometry; keys GEOM_FIELDS;
+        "heavy" is None where the pipeline did not report it)."""
+        out = (ctypes.c_uint64 * len(GEOM_FIELDS))()
+        self._ck(self.lib.pcgpu_msm_last_geometry(self.ctx, out, len(GEOM_FIELDS)))
+        g = dict(zip(GEOM_FIELDS, (int(v) for v in out)))
+        if g["heavy"] == 2**64 - 1:
+            g["heavy"] = None
+        return g
+
+    def diag_field_op(self, curve, which, op, a, b):
+        """one field primitive elementwise on the device (pcgpu_diag_field_op): which 0 = Fq, 1 = Fr of `curve`; a, b: (n, limbs)
+        uint64 Montgomery elements (limbs = 6 for BLS12-381 Fq, else 4); returns the (n, limbs) results."""
+        a, b = _u64(a), _u64(b)
+        if a.shape != b.shape:
+            raise ValueError("operand shapes differ")
+        out = np.zeros_like(a)
+        self._ck(self.lib.pcgpu_diag_field_op(self.ctx, curve, which, op, _ptr(a), _ptr(b), _ptr(out), a.shape[0]))
+        return out
 
     # ---- SRS ----
     def srs_register(self, curve, bases_xy, inf=None, n=None, flags=0):

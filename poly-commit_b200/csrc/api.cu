@@ -287,6 +287,24 @@ extern "C" int pcgpu_selftest_field(pcgpu_ctx *ctx, int curve, uint64_t seed, si
   });
 }
 
+extern "C" int pcgpu_msm_last_geometry(pcgpu_ctx *ctx, uint64_t *out, size_t len) {
+  return guarded([&]() -> int {
+  if (!ctx || (len && !out)) return PCGPU_E_BADARG;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  for (size_t i = 0; i < len && i < (size_t)PCGPU_GEOM_FIELDS; i++) out[i] = ctx->last_geom[i];
+  return PCGPU_OK;
+  });
+}
+
+extern "C" int pcgpu_diag_field_op(pcgpu_ctx *ctx, int curve, int which, int op, const void *a, const void *b, void *out, size_t n) {
+  return guarded([&]() -> int {
+  if (!ctx || (which != 0 && which != 1) || op < 0 || op > 9 || (n && (!a || !b || !out))) return PCGPU_E_BADARG;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  SET_DEVICE(ctx);
+  DISPATCH_CURVE(curve, return diag_field_op_impl<C>(ctx, which, op, a, b, out, n));
+  });
+}
+
 extern "C" uint64_t pcgpu_launch_count(void) { return rt::launch_counter().load(); }
 
 extern "C" int pcgpu_ntt(pcgpu_ctx *ctx, int curve, const void *in, size_t n_in, uint32_t logn, uint32_t flags, void *out) {

@@ -8,6 +8,7 @@
 #include <memory>
 #include <mutex>
 #include <new>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/pcgpu.h"
@@ -23,6 +24,7 @@
 #include "msm_small.cuh"
 #include "peer.cuh"
 #include "hash.cuh"
+#include "field_ops.cuh"
 
 using namespace pcgpu;
 
@@ -87,6 +89,7 @@ struct pcgpu_ctx {
   void *h_pinned = nullptr;        // page-locked landing zone of the asynchronous plane / error-word copies (PINNED_BYTES)
   rt::event_t ev_upload;           // "inputs are on the device": lets a sibling context's stream start on them
   bool ev_ok = false;
+  uint64_t last_geom[PCGPU_GEOM_FIELDS] = {0};   // path / geometry of the most recent MSM (pcgpu_msm_last_geometry)
   std::mutex mu;
 };
 static const size_t PINNED_BYTES = 512 * 192 + 256;   // PCGPU_MAX_PLANES XYZZ<Bls12381> points + the error word
@@ -209,6 +212,8 @@ int msm_small_to_host(pcgpu_ctx *ctx, const MsmSmallProblem<C> *probs, uint32_t 
   // share stays at <= 1366 terms, which is what bounds its chain of dependent additions and its digit buffer)
   if (nmax > 2 * SMALL_MAX_N) return PCGPU_E_BADARG;
   const uint32_t split = nmax > SMALL_MAX_N ? 2 * SMALL_SPLIT : (nmax >= SMALL_SPLIT_MIN_N ? SMALL_SPLIT : 1);
+  memset(ctx->last_geom, 0, sizeof ctx->last_geom);
+  ctx->last_geom[PCGPU_GEOM_PATH] = PCGPU_MSM_PATH_SMALL; ctx->last_geom[PCGPU_GEOM_SPLIT] = split; ctx->last_geom[PCGPU_GEOM_N] = nmax;
   const size_t npts = (size_t)nprob * W * split;
   if ((rc = ctx->msm_arena.reserve(rt::Arena::pad(npts * sizeof(XYZZ<C>)) + 4096))) return rc;
   uint32_t *d_err = ctx->msm_arena.take<uint32_t>(16);
@@ -271,6 +276,11 @@ int msm_device_planes(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, 
     while (R < 8 && (avg >> R) >= 4 && (entries >> (R + 1)) >= 16 * Tmax) R++;
     if (const char *e = getenv("PCGPU_MSM_AFFINE_ROUNDS")) { int v = atoi(e); if (v >= 0 && v <= 12) R = (uint32_t)v; }
     g.affine_rounds = R;
+    uint64_t *lg = ctx->last_geom;
+    memset(lg, 0, sizeof ctx->last_geom);
+    lg[PCGPU_GEOM_PATH] = PCGPU_MSM_PATH_BUCKETS; lg[PCGPU_GEOM_N] = g.n; lg[PCGPU_GEOM_C] = g.c; lg[PCGPU_GEOM_W] = g.W;
+    lg[PCGPU_GEOM_G] = g.G; lg[PCGPU_GEOM_R] = R; lg[PCGPU_GEOM_WAVE] = Tmax; lg[PCGPU_GEOM_ENTRIES] = entries;
+    lg[PCGPU_GEOM_HEAVY] = UINT64_MAX;   // msm_collect fills it in from the pipeline's error words
   }
   if (g.affine_rounds && !ctx->d_pow2[C::ID]) {
     using QP = typename C::Fq;
@@ -278,7 +288,10 @@ int msm_device_planes(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, 
     if ((rc = rt::launch<32>(Pow2TableBody<QP>{ctx->d_pow2[C::ID]}, 1, st))) return rc;
   }
   *g_out = g;
-  return msm_run<C>(tables, g, d_scalars, ctx->msm_arena, d_planes, stride, d_err, st, ctx->prof, ctx->d_pow2[C::ID]);
+  uint32_t T = 0, tdiv = 0;
+  rc = msm_run<C>(tables, g, d_scalars, ctx->msm_arena, d_planes, stride, d_err, st, ctx->prof, ctx->d_pow2[C::ID], &T, &tdiv);
+  ctx->last_geom[PCGPU_GEOM_T] = T; ctx->last_geom[PCGPU_GEOM_TDIV] = tdiv;
+  return rc;
 }
 
 // One MSM in two halves so that a caller can keep several pipelines in flight from one host thread:
@@ -299,7 +312,7 @@ int msm_issue(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, const ui
               MsmPending<C> *p) {
   rt::stream_t st = ctx->stream;
   p->done = true; p->ready = host::HXYZZ<C>::inf(); p->np = 0;
-  if (n == 0) return PCGPU_OK;
+  if (n == 0) { memset(ctx->last_geom, 0, sizeof ctx->last_geom); return PCGPU_OK; }
   if (n <= SMALL_MAX_N && msm_small_enabled()) {
     MsmSmallProblem<C> pr{(const Affine<C> *)srs->d_tables + base_offset, d_scalars, nullptr, nullptr, (uint32_t)n};
     return msm_small_to_host<C>(ctx, &pr, 1, mont, &p->ready);
@@ -312,7 +325,7 @@ int msm_issue(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, const ui
   if (p->np > PCGPU_MAX_PLANES || !ctx->h_pinned) return PCGPU_E_BADARG;
   char *hp = (char *)ctx->h_pinned;
   if ((rc = rt::copy_d2h_2d(hp, sizeof(XYZZ<C>), d_planes, stride * sizeof(XYZZ<C>), sizeof(XYZZ<C>), p->np, st))) return rc;
-  if ((rc = rt::copy_d2h(hp + PINNED_BYTES - 64, d_err, sizeof(uint32_t), st))) return rc;
+  if ((rc = rt::copy_d2h(hp + PINNED_BYTES - 64, d_err, 16 * sizeof(uint32_t), st))) return rc;   // all of msm_run's error words
   p->done = false;
   return PCGPU_OK;
 }
@@ -324,9 +337,10 @@ int msm_collect(pcgpu_ctx *ctx, MsmPending<C> *p, host::HXYZZ<C> *out) {
   if (rc) return rc;
   ctx->prof.collect();
   const char *hp = (const char *)ctx->h_pinned;
-  uint32_t herr;
-  memcpy(&herr, hp + PINNED_BYTES - 64, sizeof herr);
-  if (herr) return PCGPU_E_RANGE;
+  uint32_t herr[16];
+  memcpy(herr, hp + PINNED_BYTES - 64, sizeof herr);
+  ctx->last_geom[PCGPU_GEOM_HEAVY] = herr[12];   // err[12]: heavy buckets (msm_run)
+  if (herr[0]) return PCGPU_E_RANGE;
   auto t0 = std::chrono::steady_clock::now();
   const host::HXYZZ<C> *planes = (const host::HXYZZ<C> *)hp;
   *out = p->g.h_split ? host::combine_bit_planes_2level<C>(planes, p->g.S, p->g.c, p->g.h_split)
@@ -1440,6 +1454,39 @@ struct FieldSelfTestBody {
   }
 };
 
+// pcgpu_diag_field_op: FieldOpBody on the device, host operands staged through the context's arena
+template <class C, class P>
+static int diag_field_op_run(pcgpu_ctx *ctx, int op, const void *a, const void *b, void *out, size_t n) {
+  rt::stream_t st = ctx->stream;
+  const size_t bytes = n * P::N * 4, tbytes = (size_t)(64 * P::N + 1) * P::N * 4;
+  int rc;
+  if ((rc = ctx->stage.reserve(3 * rt::Arena::pad(bytes) + rt::Arena::pad(tbytes) + 4096))) return rc;
+  uint32_t *da = ctx->stage.take<uint32_t>(n * P::N), *db = ctx->stage.take<uint32_t>(n * P::N);
+  uint32_t *dout = ctx->stage.take<uint32_t>(n * P::N);
+  const uint32_t *pow2 = nullptr;
+  if (op == 8) {
+    if (std::is_same<P, typename C::Fq>::value) {   // the table the pair rounds use
+      if ((rc = ensure_pow2<C>(ctx))) return rc;
+      pow2 = ctx->d_pow2[C::ID];
+    } else {                                         // no kernel inverts in Fr by binary GCD: a table for this call only
+      uint32_t *t = ctx->stage.take<uint32_t>(tbytes / 4);
+      if ((rc = rt::launch<32>(Pow2TableBody<P>{t}, 1, st))) return rc;
+      pow2 = t;
+    }
+  }
+  if ((rc = rt::copy_h2d(da, a, bytes, st)) || (rc = rt::copy_h2d(db, b, bytes, st))) return rc;
+  if ((rc = rt::launch<128>(FieldOpBody<P>{da, db, dout, pow2, op}, n, st))) return rc;
+  if ((rc = rt::copy_d2h(out, dout, bytes, st))) return rc;
+  return rt::stream_sync(st);
+}
+
+template <class C>
+int diag_field_op_impl(pcgpu_ctx *ctx, int which, int op, const void *a, const void *b, void *out, size_t n) {
+  if (n == 0) return PCGPU_OK;
+  return which == 0 ? diag_field_op_run<C, typename C::Fq>(ctx, op, a, b, out, n)
+                    : diag_field_op_run<C, typename C::Fr>(ctx, op, a, b, out, n);
+}
+
 template <class C>
 int selftest_field_impl(pcgpu_ctx *ctx, uint64_t seed, size_t n, uint64_t *mismatches) {
   rt::stream_t st = ctx->stream;
@@ -1550,6 +1597,7 @@ inline int measure_imad_peak_impl(pcgpu_ctx *ctx, double *ops_per_s) {
   EXT template int fr_row_mul_impl<C>(pcgpu_ctx *, const void *, const void *, size_t, size_t, void *, uint32_t);          \
   EXT template int fr_mul_impl<C>(pcgpu_ctx *, const void *, const void *, void *, size_t, uint32_t); \
   EXT template int selftest_field_impl<C>(pcgpu_ctx *, uint64_t, size_t, uint64_t *); \
+  EXT template int diag_field_op_impl<C>(pcgpu_ctx *, int, int, const void *, const void *, void *, size_t); \
   EXT template int ntt_impl<C>(pcgpu_ctx *, const void *, size_t, uint32_t, uint32_t, void *); \
   EXT template int ntt_pass_impl<C>(pcgpu_ctx *, uint32_t, uint32_t, int, size_t, size_t, const void *, size_t, void *); \
   EXT template int ntt_batch_impl<C>(pcgpu_ctx *, const void *, size_t, size_t, uint32_t, uint32_t, void *); \

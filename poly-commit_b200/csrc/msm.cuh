@@ -630,10 +630,11 @@ int msm_reduce_launch(const MsmGeom &g, const uint32_t *task_off, const XYZZ<C> 
 // Runs the device pipeline on `st`.  d_scalars: n x 8 uint32 on the device.  On return (asynchronously)
 // *d_planes points at the S*c bit-plane sums, element (s*c + j) at index (s*c + j) * plane_stride, and
 // *d_err at a device word that is non-zero when a scalar was out of range.  `prof` brackets stages with events.
+// *pair_threads / *pair_tdiv (if given) receive the pair-round kernel's thread count and wave divisor (0 without rounds).
 template <class C, class Prof>
 inline int msm_run(const uint32_t *tables, const MsmGeom &g, const uint32_t *d_scalars, rt::Arena &arena,
                    const XYZZ<C> **d_planes, size_t *plane_stride, uint32_t **d_err_out, rt::stream_t st, Prof &prof,
-                   const uint32_t *pow2 = nullptr) {
+                   const uint32_t *pow2 = nullptr, uint32_t *pair_threads = nullptr, uint32_t *pair_tdiv = nullptr) {
   int rc;
   if ((rc = arena.reserve(msm_workspace_bytes<C>(g)))) return rc;
   size_t max_entries = (size_t)g.n * g.W;
@@ -691,6 +692,8 @@ inline int msm_run(const uint32_t *tables, const MsmGeom &g, const uint32_t *d_s
     uint32_t tdiv = g.pair_tdiv ? g.pair_tdiv : 1;
     if (const char *e = getenv("PCGPU_MSM_AFFINE_TDIV")) { int v = atoi(e); if (v >= 1 && v <= 16) tdiv = (uint32_t)v; }  // tuning knob
     if (tdiv > 1) Tmax = (Tmax / tdiv + 127) / 128 * 128;
+    if (pair_threads) *pair_threads = (uint32_t)Tmax;
+    if (pair_tdiv) *pair_tdiv = tdiv;
     prof.begin(11, st);
     const uint32_t *off_in = offsets;
     size_t bound = max_entries;

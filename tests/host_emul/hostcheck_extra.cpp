@@ -3,7 +3,7 @@
 // multiplier and the Python big-integer oracle.
 #include <stddef.h>
 #include <vector>
-#include "../../poly-commit_b200/csrc/ec.cuh"
+#include "../../poly-commit_b200/csrc/field_ops.cuh"
 using namespace pcgpu;
 
 template <class P>
@@ -13,28 +13,11 @@ static const uint32_t *pow2_table() {
   return t.data();
 }
 
+// the op switch is FieldOpBody (csrc/field_ops.cuh), the body pcgpu_diag_field_op launches on the device
 template <class P>
 static void mul_many(const uint32_t *a, const uint32_t *b, uint32_t *out, size_t n, int which) {
-  for (size_t i = 0; i < n; i++) {
-    Fp<P> x, y, r;
-    for (int j = 0; j < P::N; j++) { x.l[j] = a[i * P::N + j]; y.l[j] = b[i * P::N + j]; }
-    switch (which) {
-      case 0: r = mont_mul<P>(x, y); break;
-      case 1: r = mont_mul_ref<P>(x, y); break;
-      case 2: r = fp_add<P>(x, y); break;
-      case 3: r = fp_sub<P>(x, y); break;
-      case 4: r = fp_neg<P>(x); break;
-      case 5: r = fp_inv<P>(x); break;
-      case 8: r = fp_inv_gcd<P>(x, pow2_table<P>()); break;
-      case 9: r = mont_sqr<P>(x); break;
-      case 6: if constexpr (mont_mul2_supported<P>()) r = mont_mul2<P>(x, y, y, fp_neg<P>(x)); else r = Fp<P>::zero(); break;  // x*y + y*(-x) = 0
-      case 7: if constexpr (mont_mul2_supported<P>()) r = mont_mul2<P>(x, y, fp_add<P>(x, y), fp_sub<P>(y, x));
-              else r = fp_add<P>(mont_mul<P>(x, y), mont_mul<P>(fp_add<P>(x, y), fp_sub<P>(y, x)));
-              break;  // x*y + (x+y)(y-x)
-      default: r = Fp<P>::zero();
-    }
-    for (int j = 0; j < P::N; j++) out[i * P::N + j] = r.l[j];
-  }
+  const FieldOpBody<P> body{a, b, out, pow2_table<P>(), which};
+  for (size_t i = 0; i < n; i++) body(i);
 }
 
 // field: 0 bls Fq, 1 bls Fr, 2 bn Fq, 3 bn Fr, 4 pallas Fq, 5 pallas Fr

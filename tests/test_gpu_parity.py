@@ -19,7 +19,10 @@ from tests.test_hostcheck import (test_fixed_base_mul, test_fr_div_linear, test_
                                   test_wire_roundtrip_vs_oracle, test_wire_bls12_381_generator_known_answer,
                                   test_wire_rejects_like_the_oracle, test_wire_kzg_containers, test_msm_bases_unregistered,
                                   test_kzg10_batch_check_combination, test_ligero_reed_solomon_like_the_reference, test_msm_small_path_limits, test_ipa_fold_glv_equals_plain_ladder, test_sonic_pc_host_mirror,
-                                  test_ligero_compute_matrices, test_kzg_commit_open_fused, test_ipa_frozen_key_rounds, test_marlin_pc_hiding_and_bounds, test_sample_generators, test_ntt_batch_long_rows)
+                                  test_ligero_compute_matrices, test_kzg_commit_open_fused, test_ipa_frozen_key_rounds, test_marlin_pc_hiding_and_bounds, test_sample_generators, test_ntt_batch_long_rows,
+                                  test_field_schedule_vs_bigint, test_msm_small_split_boundaries,
+                                  test_wire_decode_fuzz_agrees_with_the_oracle, test_empty_inputs_on_the_widened_entry_points,
+                                  test_ipa_fold_special_challenges, test_ntt_pass1_with_fused_exchange)
 
 pytestmark = pytest.mark.gpu
 

@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 
 from oracle import orc, pyref
-from tests import golden_cases, util
+from tests import golden_cases, msm_cases, util
 
 FIELDS = [("bls12_381", "p", 0), ("bls12_381", "r", 1), ("bn254", "p", 2), ("bn254", "r", 3), ("pallas", "p", 4),
           ("pallas", "r", 5)]
@@ -33,6 +33,23 @@ def _dev(eng, a):
     return t.data_ptr(), t
 
 
+def _dev_zeros(eng, shape):
+    """a zero-filled uint64 buffer of `shape` that kernels write: (pointer, read-back function) -- the host array itself under
+    host emulation, a CUDA tensor on the GPU"""
+    if not msm_cases.on_gpu(eng):
+        a = np.zeros(shape, dtype=np.uint64)
+        return a.ctypes.data, lambda: a
+    import torch
+    t = torch.zeros(shape, dtype=torch.int64, device="cuda")
+    torch.cuda.synchronize()
+
+    def read():
+        torch.cuda.synchronize()
+        return t.cpu().numpy().view(np.uint64)
+    read.keep = t
+    return t.data_ptr(), read
+
+
 def _tol(vs, n64):
     out = np.zeros((len(vs), n64), dtype=np.uint64)
     for i, v in enumerate(vs):
@@ -41,44 +58,64 @@ def _tol(vs, n64):
     return out
 
 
+def _ints(arr):
+    """(n, limbs) uint64 -> list of Python ints"""
+    raw, w = np.ascontiguousarray(arr, dtype=np.uint64).tobytes(), 8 * arr.shape[1]
+    return [int.from_bytes(raw[i:i + w], "little") for i in range(0, len(raw), w)]
+
+
+def _field_operands(mod, n64, R, g, n_random):
+    """operand pairs (a, b) in Montgomery form: the edge cross product; with n_random > 400 (the device) additionally values
+    whose 32-bit limbs are 0, 1, 2^31 or 2^32-1, p - 2^(32k) and 2^(32k) - 1, pairs whose Montgomery product is 0, 1 or p-1,
+    and n_random uniform pairs"""
+    edge = [0, 1, 2, mod - 1, mod - 2, R, R * R % mod, mod >> 1, (mod >> 1) + 1, (1 << (mod.bit_length() - 1)),
+            (1 << (mod.bit_length() - 1)) - 1, (1 << 32) - 1, (1 << 64) - 1, ((1 << (32 * 2 * n64 - 2)) - 1) % mod]
+    va = edge + [e for e in edge for _ in edge]
+    vb = edge + [e for _ in edge for e in edge]
+    if n_random > 400:
+        n32 = 2 * n64
+        limbs = [0, 1, 1 << 31, (1 << 32) - 1]
+        pat = [sum(limbs[int(d)] << (32 * j) for j, d in enumerate(row)) % mod for row in g.integers(0, 4, size=(4096, n32))]
+        pat += [sum(v << (32 * j) for j in range(n32)) % mod for v in limbs]
+        pat += [(mod - (1 << (32 * k))) % mod for k in range(n32)] + [((1 << (32 * k)) - 1) % mod for k in range(1, n32 + 1)]
+        va += pat + pat[::-1] + pat
+        vb += pat[::-1] + pat + [edge[i % len(edge)] for i in range(len(pat))]
+        for t in (0, 1, mod - 1):                       # a * b / R == t
+            a = [int.from_bytes(g.bytes(8 * n64), "little") % (mod - 1) + 1 for _ in range(256)]
+            va += a
+            vb += [t * R % mod * pow(x, -1, mod) % mod for x in a]
+    va += [int.from_bytes(g.bytes(8 * n64), "little") % mod for _ in range(n_random)]
+    vb += [int.from_bytes(g.bytes(8 * n64), "little") % mod for _ in range(n_random)]
+    return va, vb
+
+
 @pytest.mark.parametrize("cname,which,fid", FIELDS)
-def test_field_schedule_vs_bigint(hostcheck_path, cname, which, fid):
-    lib = ctypes.CDLL(hostcheck_path)
+def test_field_schedule_vs_bigint(eng, cname, which, fid):
+    """every field primitive (FieldOpBody, csrc/field_ops.cuh: the production schedules, the 64-bit reference multiplier, both
+    inverses) through pcgpu_diag_field_op against Python integers: under host emulation with the PTX carry flags modelled in
+    C++, on the device with the real ones and 2^18 random pairs per op on top of the edge operands."""
     C = pyref.Curve(cname)
     mod = getattr(C, which)
     n64 = (mod.bit_length() + 63) // 64
     R = (1 << (64 * n64)) % mod
     Rinv = pow(R, -1, mod)
-    g = np.random.default_rng(fid)
-    edge = [0, 1, 2, mod - 1, mod - 2, R, R * R % mod, mod >> 1, (mod >> 1) + 1, (1 << (mod.bit_length() - 1)),
-            (1 << (mod.bit_length() - 1)) - 1, (1 << 32) - 1, (1 << 64) - 1, ((1 << (32 * 2 * n64 - 2)) - 1) % mod]
-    rnd = [int.from_bytes(g.bytes(8 * n64), "little") % mod for _ in range(400)]
-    va = edge + [e for e in edge for _ in edge] + rnd
-    vb = edge + [e for _ in edge for e in edge] + rnd[::-1]
+    va, vb = _field_operands(mod, n64, R, np.random.default_rng(fid), (1 << 18) if msm_cases.on_gpu(eng) else 400)
     A, B = _tol(va, n64), _tol(vb, n64)
+    fsel = 0 if which == "p" else 1
     ops = [(0, lambda a, b: a * b * Rinv % mod), (1, lambda a, b: a * b * Rinv % mod), (2, lambda a, b: (a + b) % mod),
            (3, lambda a, b: (a - b) % mod), (4, lambda a, b: (-a) % mod), (6, lambda a, b: 0),
            (7, lambda a, b: (a * b + (a + b) * (b - a)) * Rinv % mod),   # 6, 7: sum of two products, one reduction
            (9, lambda a, b: a * a * Rinv % mod)]                          # dedicated squaring
-    vp = ctypes.c_void_p
     for op, fn in ops:
-        out = np.zeros_like(A)
-        assert lib.hostcheck_field_op(fid, op, A.ctypes.data_as(vp), B.ctypes.data_as(vp), out.ctypes.data_as(vp),
-                                      ctypes.c_size_t(len(va))) == 0
-        exp = _tol([fn(a, b) for a, b in zip(va, vb)], n64)
-        assert (out == exp).all(), (cname, which, op)
-    k = 24
-    out = np.zeros_like(A[:k])
-    lib.hostcheck_field_op(fid, 5, A[:k].ctypes.data_as(vp), B[:k].ctypes.data_as(vp), out.ctypes.data_as(vp), ctypes.c_size_t(k))
-    exp = _tol([(pow(a * Rinv % mod, -1, mod) * R % mod) if a else 0 for a in va[:k]], n64)
-    assert (out == exp).all()
-    # binary-GCD (almost Montgomery) inverse == Fermat inverse, on edge values and random ones
-    k2 = 120
-    sel = list(range(len(edge))) + list(range(len(va) - k2, len(va)))
-    A2 = np.ascontiguousarray(A[sel]); out = np.zeros_like(A2)
-    lib.hostcheck_field_op(fid, 8, A2.ctypes.data_as(vp), A2.ctypes.data_as(vp), out.ctypes.data_as(vp), ctypes.c_size_t(len(sel)))
-    exp = _tol([(pow(va[i] * Rinv % mod, -1, mod) * R % mod) if va[i] else 0 for i in sel], n64)
-    assert (out == exp).all()
+        got = _ints(eng.diag_field_op(C.id, fsel, op, A, B))
+        bad = [i for i, (x, a, b) in enumerate(zip(got, va, vb)) if x != fn(a, b)]
+        assert not bad, (cname, which, op, len(bad), hex(va[bad[0]]), hex(vb[bad[0]]))
+    # inverses (Fermat and binary GCD): out = R^2 / a, i.e. a * out == R^2 (mod p) with out < p; 0 -> 0
+    RR = R * R % mod
+    for op in (5, 8):
+        got = _ints(eng.diag_field_op(C.id, fsel, op, A, A))
+        bad = [i for i, (x, a) in enumerate(zip(got, va)) if x >= mod or (a * x % mod != RR if a else x)]
+        assert not bad, (cname, which, op, len(bad), hex(va[bad[0]]))
 
 
 @pytest.mark.parametrize("cname", util.CURVE_NAMES)
@@ -153,6 +190,7 @@ def test_msm_batched_affine_rounds(eng, pc, rounds, monkeypatch):
         sc[20:40] = sc[20]                                          # a crowded bucket in every window
         srs = eng.srs_register(C.id, bases, inf=inf)
         got = eng.msm(srs, sc)
+        msm_cases.check_geometry(eng, pc, cname, bases.shape[0])          # R rounds ran
         exp = orc.msm(C.id, bases, sc, inf=inf)
         assert got[1] == exp[1] and (got[0] == exp[0]).all(), (cname, rounds)
     if rounds != 3:
@@ -163,6 +201,7 @@ def test_msm_batched_affine_rounds(eng, pc, rounds, monkeypatch):
     sc = util.rand_fr("bn254", 4200, seed=96, mont=False)
     srs = eng.srs_register(C.id, bases, flags=pc.SRS_PRECOMPUTE)
     got = eng.msm(srs, sc); exp = orc.msm(C.id, bases, sc)
+    msm_cases.check_geometry(eng, pc, "bn254", 4200, folded_c=msm_cases.srs_precompute_window(4200))
     assert (got[0] == exp[0]).all()
 
 
@@ -182,10 +221,12 @@ def test_msm_two_level_reduction(eng, pc, c, monkeypatch):
     exp = orc.msm(C.id, bases, sc)
     srs = eng.srs_register(C.id, bases[:60])
     got = eng.msm(srs, sc[:60])
+    assert eng.msm_last_geometry()["c"] == c
     assert (got[0] == orc.msm(C.id, bases[:60], sc[:60])[0]).all()
     if c == 18:
         srs = eng.srs_register(C.id, bases, flags=pc.SRS_PRECOMPUTE)
         got = eng.msm(srs, sc)
+        msm_cases.check_geometry(eng, pc, cname, n, folded_c=c)
         assert (got[0] == exp[0]).all()
 
 
@@ -203,8 +244,37 @@ def test_msm_heavy_buckets(eng, pc, rounds, monkeypatch):
     sc = C.fr_to_limbs(vals, False)
     srs = eng.srs_register(C.id, bases)
     got = eng.msm(srs, sc)
+    g = msm_cases.check_geometry(eng, pc, cname, n)
+    distinct = sorted(set(vals))
+    heavy = msm_cases.expected_heavy_buckets(cname, distinct, [vals.count(v) for v in distinct], g["c"], g["W"], g["W"], g["R"], 32)
+    assert g["heavy"] == heavy and (heavy > 0 or rounds != "0"), (g, heavy)   # two pair rounds shrink every bucket below the bar
     exp = orc.msm(C.id, bases, sc)
     assert got[1] == exp[1] and (got[0] == exp[0]).all()
+
+
+@pytest.mark.parametrize("cname", util.CURVE_NAMES)
+def test_msm_forced_depth(eng, pc, cname, monkeypatch):
+    """forced pair rounds 1 / 3 / 5 with a full and a 1/16 wave of pair threads, raw bases (n = 2001) and window-folded
+    tables (n = 4200): the case body test_gpu_msm_paths.py runs at 2^17 on the device"""
+    msm_cases.forced_depth_case(eng, pc, cname, util.random_points(cname, 2001, seed=120), monkeypatch, folded=(False,))
+    if cname == "bn254":
+        msm_cases.forced_depth_case(eng, pc, cname, util.random_points(cname, 4200, seed=121), monkeypatch, rounds=(1, 3),
+                                    folded=(True,))
+
+
+@pytest.mark.parametrize("cname", util.CURVE_NAMES)
+@pytest.mark.parametrize("rounds,tdiv", [(3, 16), (None, None)])
+def test_msm_exceptional_pairs_at_depth(eng, pc, cname, rounds, tdiv, monkeypatch):
+    """a few dozen points, their negations and identity entries repeated throughout the bases, scalars from a small set:
+    P + P, P + (-P) and identity operands at every chain position of every pair round, and an exact sum of zero"""
+    msm_cases.exceptional_case(eng, pc, cname, 2000, monkeypatch, rounds=rounds, tdiv=tdiv)
+
+
+def test_msm_heavy_buckets_past_the_grid_stride(eng, pc, monkeypatch):
+    """more heavy buckets than the heavy-bucket kernel has blocks (HEAVY_GRID): 120 distinct scalars over 4500 terms, with
+    accumulate tasks of 4 entries and no pair rounds so that the threshold is reached at emulation size"""
+    monkeypatch.setenv("PCGPU_MSM_AFFINE_ROUNDS", "0")
+    msm_cases.heavy_case(eng, pc, "bn254", util.random_points("bn254", 4500, seed=122), 120, monkeypatch, L=4)
 
 
 def test_msm_infinity_bases(eng, msm_path):
@@ -1136,36 +1206,38 @@ def test_host_tail_field_product_vs_bigint(hostcheck_path, cname, which, fid):
 def test_ntt_pass1_with_fused_exchange(eng, cname, logn, world):
     """pcgpu_ntt_pass1_peer: every "rank" transforms its columns and stores straight into the owners' row buffers (the fused
     all-to-all); pass 2 on each buffer then yields the same transform as the single call.  Ranks are simulated in-process:
-    under emulation a device pointer is a host pointer, so the peer table is just the list of buffers."""
+    under emulation a device pointer is a host pointer, so the peer table is just the list of buffers; on the GPU every
+    buffer is device memory of the one device (all "peers" are local)."""
     C = pyref.Curve(cname)
     m1, m2 = eng.ntt_split(logn)
     N1, N2 = 1 << m1, 1 << m2
     rows, cols = N1 // world, N2 // world
     n_in = (1 << logn) - 5
     x = util.rand_fr(cname, n_in, seed=200 + logn, mont=True)
+    xp, _keep = _dev(eng, x)
     for inverse in (False, True):
-        rowbufs = [np.zeros((rows, N2, 4), dtype=np.uint64) for _ in range(world)]
-        ptrs = [b.ctypes.data for b in rowbufs]
+        rowbufs = [_dev_zeros(eng, (rows, N2, 4)) for _ in range(world)]
+        ptrs = [p for p, _ in rowbufs]
         for r in range(world):
-            eng.ntt_pass1_peer(C.id, logn, r * cols, cols, x.ctypes.data, n_in, ptrs, inverse=inverse)
+            eng.ntt_pass1_peer(C.id, logn, r * cols, cols, xp, n_in, ptrs, inverse=inverse)
         outs = []
         for r in range(world):
-            o = np.zeros((N2, rows, 4), dtype=np.uint64)
-            eng.ntt_pass(C.id, logn, 2, r * rows, rows, rowbufs[r].ctypes.data, rows * N2, o.ctypes.data, inverse=inverse)
-            outs.append(o)
-        got = np.stack(outs, 0).transpose(1, 0, 2, 3).reshape(-1, 4)
+            o, read = _dev_zeros(eng, (N2, rows, 4))
+            eng.ntt_pass(C.id, logn, 2, r * rows, rows, ptrs[r], rows * N2, o, inverse=inverse)
+            outs.append(read)
+        got = np.stack([read() for read in outs], 0).transpose(1, 0, 2, 3).reshape(-1, 4)
         assert (got == eng.ntt(C.id, x, logn, inverse=inverse)).all()
     # the host-side driver (one engine per "device")
     from poly_commit_b200 import sharded
     pn = sharded.PeerNtt([eng] * world, C.id, logn)
-    rowbufs = [np.zeros((rows, N2, 4), dtype=np.uint64) for _ in range(world)]
-    outs = [np.zeros((N2, rows, 4), dtype=np.uint64) for _ in range(world)]
-    pn.forward([x.ctypes.data] * world, n_in, [b.ctypes.data for b in rowbufs], [o.ctypes.data for o in outs])
-    assert (np.stack(outs, 0).transpose(1, 0, 2, 3).reshape(-1, 4) == eng.ntt(C.id, x, logn)).all()
+    rowbufs = [_dev_zeros(eng, (rows, N2, 4)) for _ in range(world)]
+    outs = [_dev_zeros(eng, (N2, rows, 4)) for _ in range(world)]
+    pn.forward([xp] * world, n_in, [p for p, _ in rowbufs], [p for p, _ in outs])
+    assert (np.stack([read() for _, read in outs], 0).transpose(1, 0, 2, 3).reshape(-1, 4) == eng.ntt(C.id, x, logn)).all()
     with pytest.raises(Exception):
-        eng.ntt_pass1_peer(C.id, logn, 0, cols, x.ctypes.data, n_in, [ptrs[0]] * 3)        # 3 ranks do not divide N1
+        eng.ntt_pass1_peer(C.id, logn, 0, cols, xp, n_in, [ptrs[0]] * 3)        # 3 ranks do not divide N1
     with pytest.raises(Exception):
-        eng.ntt_pass1_peer(C.id, logn, N2 - 1, 2, x.ctypes.data, n_in, ptrs)                # columns out of range
+        eng.ntt_pass1_peer(C.id, logn, N2 - 1, 2, xp, n_in, ptrs)                # columns out of range
 
 
 def test_sonic_pc_host_mirror(eng, pc):
