@@ -71,7 +71,7 @@ int pcgpu_set_stream(pcgpu_ctx *ctx, void *cuda_stream);
 /* Per-stage device timings (CUDA events on the launching stream).  stage: 0 digits/count, 1 scan,
  * 2 scatter, 3 tasks, 4 bucket accumulate (XYZZ), 5 bucket reduce, 6 final (host tail, wall clock), 7 fr division,
  * 8 fr axpy, 9 ntt, 10 comb batch, 11 affine pair rounds (all), 12 affine pair round 0 kernel alone, 13 peer push + wait,
- * 14 column hashes + Merkle tree.
+ * 14 column hashes + Merkle tree, 15 Brakedown encoding.
  * enable=1 starts recording; get returns accumulated milliseconds and launch count since enable. */
 int pcgpu_profile_enable(pcgpu_ctx *ctx, int enable);
 int pcgpu_profile_get(pcgpu_ctx *ctx, int stage, double *ms, uint64_t *count);
@@ -219,6 +219,36 @@ int pcgpu_lincode_hash_columns(pcgpu_ctx *ctx, int curve, const void *ext_mat, s
 int pcgpu_merkle_tree(pcgpu_ctx *ctx, const uint8_t *leaves, size_t n_leaves, uint32_t flags, uint8_t *out_nodes, uint8_t *out_root);
 int pcgpu_lincode_commit(pcgpu_ctx *ctx, int curve, const void *mat, size_t n_rows, size_t n_cols, uint32_t log_ext_cols, int hash,
                          uint32_t flags, void *out_ext_mat, uint8_t *out_leaves, uint8_t *out_nodes, uint8_t *out_root);
+
+/* ---- Brakedown (MultilinearBrakedown, linear_codes/brakedown.rs + multilinear_brakedown/mod.rs) ------------------------
+ * pcgpu_brakedown_register: the code of a BrakedownPCParams (brakedown.rs:146-203), uploaded once: m message columns,
+ *   m_ext codeword columns, `levels` L, a_dims / b_dims as L (rows, cols, nonzeros per row) triples each, and 2L CSC matrices
+ *   A_0..A_{L-1}, B_0..B_{L-1} exactly as SprsMat stores them (linear_codes/utils.rs:20-107): ind_ptr[cols + 1] and
+ *   col_ind[ind_ptr[cols]] u64, val[ind_ptr[cols]] Montgomery Fr.  The matrices come from the caller's RNG (make_mat,
+ *   brakedown.rs:305-333), so they are data here, like an SRS.  Checked on the host: PCGPU_E_BADARG when a_dims[0].0 != m,
+ *   a_dims[i].1 != a_dims[i+1].0, b_dims[i].0 != end[i] - start[i], m_ext != codeword_len (brakedown.rs:292-299; with L = 0,
+ *   m_ext < m), the Reed-Solomon output is shorter than its input, an ind_ptr does not start at 0, is not monotone or exceeds
+ *   rows * nonzeros, or a col_ind >= rows; PCGPU_E_RANGE when a value is not a reduced field element.  At most 16 levels.
+ * pcgpu_brakedown_encode: MultilinearBrakedown::encode (multilinear_brakedown/mod.rs:56-84) of every row of `mat`
+ *   (n_rows x n_cols, row-major) -> out_ext (n_rows x m_ext, row-major, compute_matrices' ext_mat).  n_cols != m:
+ *   PCGPU_E_LEN (Error::EncodingError).
+ * pcgpu_brakedown_commit: encode + column hashes + Merkle tree without leaving the device, like pcgpu_lincode_commit (the tree
+ *   pads m_ext leaves to a power of two with empty leaves); out_ext, out_leaves (m_ext x 32) and out_nodes may be NULL.
+ * pcgpu_fr_sprs_row_mul: SprsMat::row_mul (utils.rs:41-52) of an n x m CSC matrix on `count` vectors (count x n, row-major)
+ *   -> out (count x m).  The matrix arrays are host pointers (checked as above, without a nonzero bound).
+ * With PCGPU_DEVICE_PTRS the matrix / vector / output arguments (not the CSC arrays) are device pointers.  Profile stage 15 is
+ * the encoding; the hashes and the tree are stage 14. */
+typedef struct pcgpu_brakedown pcgpu_brakedown;
+int pcgpu_brakedown_register(pcgpu_ctx *ctx, int curve, size_t m, size_t m_ext, size_t levels, const uint64_t *a_dims,
+                             const uint64_t *b_dims, const uint64_t *const *ind_ptr, const uint64_t *const *col_ind,
+                             const void *const *val, uint32_t flags, pcgpu_brakedown **out);
+void pcgpu_brakedown_release(pcgpu_ctx *ctx, pcgpu_brakedown *code);
+int pcgpu_brakedown_encode(pcgpu_ctx *ctx, const pcgpu_brakedown *code, const void *mat, size_t n_rows, size_t n_cols, uint32_t flags,
+                           void *out_ext);
+int pcgpu_brakedown_commit(pcgpu_ctx *ctx, const pcgpu_brakedown *code, const void *mat, size_t n_rows, size_t n_cols, int hash,
+                           uint32_t flags, void *out_ext, uint8_t *out_leaves, uint8_t *out_nodes, uint8_t *out_root);
+int pcgpu_fr_sprs_row_mul(pcgpu_ctx *ctx, int curve, size_t n, size_t m, const uint64_t *ind_ptr, const uint64_t *col_ind,
+                          const void *val, const void *v, size_t count, uint32_t flags, void *out);
 
 /* ---- multi-GPU over NVLink peer memory (SURVEY.md section 8e) -------------------------------------------------------
  * One process per GPU.  Every rank allocates ONE window (pcgpu_peer_window_bytes() bytes, zero-filled) with pcgpu_peer_alloc,

@@ -114,6 +114,12 @@ def _load(path):
         "pcgpu_lincode_hash_columns": [_vp, ctypes.c_int, _vp, _sz, _sz, ctypes.c_int, ctypes.c_uint32, _vp],
         "pcgpu_merkle_tree": [_vp, _vp, _sz, ctypes.c_uint32, _vp, _vp],
         "pcgpu_lincode_commit": [_vp, ctypes.c_int, _vp, _sz, _sz, ctypes.c_uint32, ctypes.c_int, ctypes.c_uint32, _vp, _vp, _vp, _vp],
+        "pcgpu_brakedown_register": [_vp, ctypes.c_int, _sz, _sz, _sz, _vp, _vp, ctypes.POINTER(_vp), ctypes.POINTER(_vp),
+                                     ctypes.POINTER(_vp), ctypes.c_uint32, ctypes.POINTER(_vp)],
+        "pcgpu_brakedown_release": [_vp, _vp],
+        "pcgpu_brakedown_encode": [_vp, _vp, _vp, _sz, _sz, ctypes.c_uint32, _vp],
+        "pcgpu_brakedown_commit": [_vp, _vp, _vp, _sz, _sz, ctypes.c_int, ctypes.c_uint32, _vp, _vp, _vp, _vp],
+        "pcgpu_fr_sprs_row_mul": [_vp, ctypes.c_int, _sz, _sz, _vp, _vp, _vp, _vp, _sz, ctypes.c_uint32, _vp],
         "pcgpu_peer_alloc": [_vp, _sz, ctypes.POINTER(_vp), _vp],
         "pcgpu_peer_open": [_vp, _vp, ctypes.POINTER(_vp)],
         "pcgpu_peer_close": [_vp, _vp],
@@ -128,7 +134,7 @@ def _load(path):
         if fn is None:      # a library older than this binding: only the calls that need the symbol fail (AttributeError)
             continue
         fn.argtypes = args
-        fn.restype = None if name in ("pcgpu_destroy", "pcgpu_srs_release") else ctypes.c_int
+        fn.restype = None if name in ("pcgpu_destroy", "pcgpu_srs_release", "pcgpu_brakedown_release") else ctypes.c_int
     return lib
 
 
@@ -166,6 +172,32 @@ class Srs:
             self.release()
         except Exception:
             pass
+
+
+class BrakedownCode:
+    """Device-resident code of a BrakedownPCParams (its 2L sparse matrices); m / m_ext are the row lengths before and after
+    encoding."""
+
+    def __init__(self, engine, handle, curve, m, m_ext):
+        self.engine, self.handle, self.curve, self.m, self.m_ext = engine, handle, curve, m, m_ext
+
+    def release(self):
+        if self.handle is not None and getattr(self.engine, "ctx", None):
+            h, self.handle = self.handle, None
+            self.engine.lib.pcgpu_brakedown_release(self.engine.ctx, h)
+
+    def __del__(self):
+        try:
+            self.release()
+        except Exception:
+            pass
+
+
+def _csc_arrays(mat):
+    """(ind_ptr, col_ind, val) as the ABI takes them: u64, u64, (nnz, 4) u64 Montgomery"""
+    ind_ptr, col_ind, val = mat
+    return (np.ascontiguousarray(ind_ptr, dtype=np.uint64), np.ascontiguousarray(col_ind, dtype=np.uint64),
+            np.ascontiguousarray(np.asarray(val, dtype=np.uint64).reshape(-1, 4)))
 
 
 class DeviceBuffer:
@@ -536,6 +568,64 @@ class Engine:
         self._ck(self.lib.pcgpu_lincode_commit(self.ctx, curve, _ptr(mat), n_rows, n_cols, log_ext_cols, hash, flags, _ptr(out_ext),
                                                _ptr(out_leaves), _ptr(out_nodes), _ptr(root)))
         return dict(root=root, ext=out_ext, leaves=out_leaves, nodes=out_nodes)
+
+    # ---- Brakedown: sparse row encoding in front of the same hashes + tree ----
+    def brakedown_register(self, curve, m, m_ext, a_dims, b_dims, a_mats, b_mats, flags=0):
+        """upload a BrakedownPCParams' code: a_dims / b_dims lists of (rows, cols, nonzeros per row), a_mats / b_mats lists of
+        SprsMat as (ind_ptr, col_ind, val) -> BrakedownCode"""
+        L = len(a_dims)
+        if len(b_dims) != L or len(a_mats) != L or len(b_mats) != L:
+            raise ValueError("a_dims, b_dims, a_mats and b_mats must have one entry per level")
+        mats = [_csc_arrays(x) for x in list(a_mats) + list(b_mats)]
+        ad = np.ascontiguousarray(np.asarray(a_dims, dtype=np.uint64).reshape(-1))
+        bd = np.ascontiguousarray(np.asarray(b_dims, dtype=np.uint64).reshape(-1))
+        P = (_vp * max(1, 2 * L))(*[_ptr(x[0]) for x in mats])
+        C = (_vp * max(1, 2 * L))(*[_ptr(x[1]) for x in mats])
+        V = (_vp * max(1, 2 * L))(*[_ptr(x[2]) for x in mats])
+        h = _vp()
+        self._ck(self.lib.pcgpu_brakedown_register(self.ctx, curve, m, m_ext, L, _ptr(ad), _ptr(bd), P, C, V, flags, ctypes.byref(h)))
+        return BrakedownCode(self, h, curve, m, m_ext)
+
+    def brakedown_encode(self, code, mat, n_rows=None, n_cols=None, flags=0, out=None):
+        """MultilinearBrakedown::encode of every row of a (n_rows, m, 4) Montgomery matrix -> (n_rows, m_ext, 4)"""
+        mat = _u64(mat)
+        if n_rows is None:
+            n_rows, n_cols = mat.shape[0], mat.shape[1]
+        if out is None:
+            out = np.zeros((n_rows, code.m_ext, 4), dtype=np.uint64)
+        self._ck(self.lib.pcgpu_brakedown_encode(self.ctx, code.handle, _ptr(mat), n_rows, n_cols, flags, _ptr(out)))
+        return out
+
+    def brakedown_commit(self, code, mat, n_rows=None, n_cols=None, hash=0, flags=0, want=("ext", "leaves", "nodes"),
+                         out_ext=None, out_leaves=None, out_nodes=None):
+        """encode + column hashes + Merkle tree in one device-resident call -> dict(root, ext?, leaves?, nodes?)"""
+        mat = _u64(mat)
+        if n_rows is None:
+            n_rows, n_cols = mat.shape[0], mat.shape[1]
+        N = code.m_ext
+        P = 1 << max(1, (N - 1).bit_length())
+        if not (flags & DEVICE_PTRS):
+            out_ext = np.zeros((n_rows, N, 4), dtype=np.uint64) if "ext" in want else None
+            out_leaves = np.zeros((N, 32), dtype=np.uint8) if "leaves" in want else None
+            out_nodes = np.zeros((P - 1, 32), dtype=np.uint8) if "nodes" in want else None
+        root = np.zeros(32, dtype=np.uint8)
+        self._ck(self.lib.pcgpu_brakedown_commit(self.ctx, code.handle, _ptr(mat), n_rows, n_cols, hash, flags, _ptr(out_ext),
+                                                 _ptr(out_leaves), _ptr(out_nodes), _ptr(root)))
+        return dict(root=root, ext=out_ext, leaves=out_leaves, nodes=out_nodes)
+
+    def sprs_row_mul(self, curve, n, m, mat, v, count=None, flags=0, out=None):
+        """SprsMat::row_mul of an n x m CSC matrix (ind_ptr, col_ind, val) on `count` vectors (count, n, 4) -> (count, m, 4)"""
+        ind_ptr, col_ind, val = _csc_arrays(mat)
+        if ind_ptr.size != m + 1:
+            raise ValueError("ind_ptr must have m + 1 entries")
+        v = _u64(v)
+        if count is None:
+            count = v.size // (4 * n) if n else 0
+        if out is None:
+            out = np.zeros((count, m, 4), dtype=np.uint64)
+        self._ck(self.lib.pcgpu_fr_sprs_row_mul(self.ctx, curve, n, m, _ptr(ind_ptr), _ptr(col_ind), _ptr(val), _ptr(v), count, flags,
+                                                _ptr(out)))
+        return out
 
     # ---- multi-GPU over NVLink peer memory ----
     def peer_window_bytes(self):

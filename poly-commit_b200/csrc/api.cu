@@ -688,6 +688,78 @@ extern "C" int pcgpu_lincode_commit(pcgpu_ctx *ctx, int curve, const void *mat, 
   });
 }
 
+// ---- Brakedown (sprs.cuh) -----------------------------------------------------------------------------------------------
+extern "C" int pcgpu_brakedown_register(pcgpu_ctx *ctx, int curve, size_t m, size_t m_ext, size_t levels, const uint64_t *a_dims,
+                                        const uint64_t *b_dims, const uint64_t *const *ind_ptr, const uint64_t *const *col_ind,
+                                        const void *const *val, uint32_t flags, pcgpu_brakedown **out) {
+  (void)flags;
+  return guarded([&]() -> int {
+  if (!ctx || !out) return PCGPU_E_BADARG;
+  *out = nullptr;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  SET_DEVICE(ctx);
+  pcgpu_brakedown *bd = new (std::nothrow) pcgpu_brakedown();
+  if (!bd) return PCGPU_E_OOM;
+  bd->d_mem = nullptr;
+  int rc;
+  switch (curve) {
+    case PCGPU_BLS12_381: rc = brakedown_register_impl<Bls12381>(ctx, m, m_ext, levels, a_dims, b_dims, ind_ptr, col_ind, val, bd); break;
+    case PCGPU_BN254: rc = brakedown_register_impl<Bn254>(ctx, m, m_ext, levels, a_dims, b_dims, ind_ptr, col_ind, val, bd); break;
+    case PCGPU_PALLAS: rc = brakedown_register_impl<Pallas>(ctx, m, m_ext, levels, a_dims, b_dims, ind_ptr, col_ind, val, bd); break;
+    default: rc = PCGPU_E_BADARG;
+  }
+  if (rc) { rt::dev_free(bd->d_mem); delete bd; return rc; }
+  *out = bd;
+  return PCGPU_OK;
+  });
+}
+
+extern "C" void pcgpu_brakedown_release(pcgpu_ctx *ctx, pcgpu_brakedown *code) {
+  if (!code) return;
+  if (ctx) {
+    std::lock_guard<std::mutex> lk(ctx->mu);
+#ifndef PCGPU_EMUL
+    cudaSetDevice(ctx->device);
+    cudaStreamSynchronize(ctx->stream);
+#endif
+    rt::dev_free(code->d_mem);
+  } else {
+    rt::dev_free(code->d_mem);
+  }
+  delete code;
+}
+
+extern "C" int pcgpu_brakedown_encode(pcgpu_ctx *ctx, const pcgpu_brakedown *code, const void *mat, size_t n_rows, size_t n_cols,
+                                      uint32_t flags, void *out_ext) {
+  return guarded([&]() -> int {
+  if (!ctx || !code || !out_ext || (n_rows && n_cols && !mat)) return PCGPU_E_BADARG;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  SET_DEVICE(ctx);
+  DISPATCH_CURVE(code->curve, return brakedown_commit_impl<C>(ctx, code, mat, n_rows, n_cols, -1, flags, out_ext, nullptr, nullptr, nullptr));
+  });
+}
+
+extern "C" int pcgpu_brakedown_commit(pcgpu_ctx *ctx, const pcgpu_brakedown *code, const void *mat, size_t n_rows, size_t n_cols, int hash,
+                                      uint32_t flags, void *out_ext, uint8_t *out_leaves, uint8_t *out_nodes, uint8_t *out_root) {
+  return guarded([&]() -> int {
+  if (!ctx || !code || hash < 0 || (n_rows && n_cols && !mat)) return PCGPU_E_BADARG;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  SET_DEVICE(ctx);
+  DISPATCH_CURVE(code->curve, return brakedown_commit_impl<C>(ctx, code, mat, n_rows, n_cols, hash, flags, out_ext, out_leaves, out_nodes,
+                                                              out_root));
+  });
+}
+
+extern "C" int pcgpu_fr_sprs_row_mul(pcgpu_ctx *ctx, int curve, size_t n, size_t m, const uint64_t *ind_ptr, const uint64_t *col_ind,
+                                     const void *val, const void *v, size_t count, uint32_t flags, void *out) {
+  return guarded([&]() -> int {
+  if (!ctx || !ind_ptr || (m && count && !out) || (n && count && !v)) return PCGPU_E_BADARG;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  SET_DEVICE(ctx);
+  DISPATCH_CURVE(curve, return fr_sprs_row_mul_impl<C>(ctx, n, m, ind_ptr, col_ind, val, v, count, flags, out));
+  });
+}
+
 // ---- fused KZG10 commit + open ------------------------------------------------------------------------------------------
 static int ensure_siblings(pcgpu_ctx *ctx, size_t count) {
   std::lock_guard<std::mutex> lk(ctx->mu);

@@ -5,6 +5,7 @@
 // g++ with -DPCGPU_EMUL into tests/host_emul/libpcgpu_hostcheck.so, a unit-test harness that runs
 // the kernel bodies serially; the package never loads that library.
 #pragma once
+#include <algorithm>
 #include <memory>
 #include <mutex>
 #include <new>
@@ -24,6 +25,7 @@
 #include "msm_small.cuh"
 #include "peer.cuh"
 #include "hash.cuh"
+#include "sprs.cuh"
 #include "field_ops.cuh"
 
 using namespace pcgpu;
@@ -1332,6 +1334,256 @@ int lincode_commit_impl(pcgpu_ctx *ctx, const void *mat, size_t n_rows, size_t n
 }
 
 // ---------------------------------------------------------------------------------------------
+// Brakedown: the sparse row encoding (sprs.cuh) in front of the same column hashes + tree
+// ---------------------------------------------------------------------------------------------
+// BrakedownPCParams' code (linear_codes/brakedown.rs:146-203) on the device.  start / end as brakedown.rs:168-181; the
+// Reed-Solomon bounds as multilinear_brakedown/mod.rs:71-73 (with the unwrap_or defaults when there are no levels).
+struct pcgpu_brakedown {
+  int curve;
+  uint64_t m, m_ext, levels;
+  std::vector<uint64_t> a_dims, b_dims, start, end;   // 3L, 3L, L, L
+  uint64_t rss, rsie, rsoe;
+  uint32_t *d_mem;                                    // every matrix: ind_ptr | col_ind | val, one allocation
+  std::vector<SprsLevel> a_lev, b_lev;
+};
+
+template <class R>
+static bool fr_words_reduced(const uint32_t *w) {
+  for (int i = R::N - 1; i >= 0; i--)
+    if (w[i] != R::mod(i)) return w[i] < R::mod(i);
+  return false;
+}
+
+// Checks one SprsMat (n rows, m columns, at most nnz_cap nonzeros) and packs the nonzeros whose row index is < lim as
+// 32-bit offsets / indices + Montgomery words.  BADARG: ind_ptr not starting at 0, not monotone, past nnz_cap or 2^32;
+// col_ind >= n.  RANGE: a value that is not a reduced field element.
+template <class R>
+static int sprs_pack(uint64_t n, uint64_t m, uint64_t nnz_cap, const uint64_t *ind_ptr, const uint64_t *col_ind, const void *val,
+                     uint64_t lim, std::vector<uint32_t> &ptr, std::vector<uint32_t> &col, std::vector<uint32_t> &vals) {
+  if (!ind_ptr || ind_ptr[0] != 0) return PCGPU_E_BADARG;
+  for (uint64_t j = 0; j < m; j++)
+    if (ind_ptr[j + 1] < ind_ptr[j]) return PCGPU_E_BADARG;
+  const uint64_t nnz = ind_ptr[m];
+  if (nnz > nnz_cap || nnz >= ((uint64_t)1 << 32)) return PCGPU_E_BADARG;
+  if (nnz && (!col_ind || !val)) return PCGPU_E_BADARG;
+  const uint32_t *w = (const uint32_t *)val;
+  for (uint64_t k = 0; k < nnz; k++) {
+    if (col_ind[k] >= n) return PCGPU_E_BADARG;
+    if (!fr_words_reduced<R>(w + 8 * k)) return PCGPU_E_RANGE;
+  }
+  ptr.assign(m + 1, 0);
+  col.clear(); vals.clear();
+  for (uint64_t j = 0; j < m; j++) {
+    for (uint64_t k = ind_ptr[j]; k < ind_ptr[j + 1]; k++) {
+      if (col_ind[k] >= lim) continue;
+      col.push_back((uint32_t)col_ind[k]);
+      vals.insert(vals.end(), w + 8 * k, w + 8 * k + 8);
+    }
+    ptr[j + 1] = (uint32_t)col.size();
+  }
+  return PCGPU_OK;
+}
+
+template <class C>
+int brakedown_register_impl(pcgpu_ctx *ctx, uint64_t m, uint64_t m_ext, uint64_t L, const uint64_t *a_dims, const uint64_t *b_dims,
+                            const uint64_t *const *ind_ptr, const uint64_t *const *col_ind, const void *const *val, pcgpu_brakedown *bd) {
+  using R = typename C::Fr;
+  if (m == 0 || L > SPRS_MAX_LEVELS || (L && (!a_dims || !b_dims || !ind_ptr || !col_ind || !val))) return PCGPU_E_BADARG;
+  bd->curve = C::ID; bd->m = m; bd->m_ext = m_ext; bd->levels = L;
+  bd->a_dims.assign(a_dims, a_dims + 3 * L); bd->b_dims.assign(b_dims, b_dims + 3 * L);
+  // shapes: A_0 reads the message, A_i reads what A_{i-1} wrote, B_i reads [start[i], end[i]), m_ext = codeword_len
+  // (brakedown.rs:292-299; without levels the caller's ceil_mul(m, rho_inv), which only has to hold the message)
+  if (L) {
+    if (a_dims[0] != m) return PCGPU_E_BADARG;
+    uint64_t s = 0, cw = 0;
+    for (uint64_t i = 0; i < L; i++) {
+      if (i + 1 < L && a_dims[3 * i + 1] != a_dims[3 * (i + 1)]) return PCGPU_E_BADARG;
+      if (a_dims[3 * i + 1] == 0 || b_dims[3 * i] == 0) return PCGPU_E_BADARG;
+      s += a_dims[3 * i]; cw += a_dims[3 * i] + b_dims[3 * i + 1];
+      bd->start.push_back(s);
+    }
+    cw += b_dims[3 * (L - 1)];
+    if (m_ext != cw) return PCGPU_E_BADARG;
+    uint64_t e = m_ext;
+    for (uint64_t i = 0; i < L; i++) {
+      e -= b_dims[3 * i + 1];
+      bd->end.push_back(e);
+      if (e < bd->start[i] || b_dims[3 * i] != e - bd->start[i]) return PCGPU_E_BADARG;
+    }
+    bd->rss = bd->start.back(); bd->rsie = bd->rss + a_dims[3 * (L - 1) + 1]; bd->rsoe = bd->end.back();
+  } else {
+    if (m_ext < m) return PCGPU_E_BADARG;
+    bd->rss = 0; bd->rsie = m; bd->rsoe = m_ext;
+  }
+  if (bd->rsoe < bd->rsie) return PCGPU_E_BADARG;   // the Reed-Solomon step must have room for its input
+  // pack: A_0..A_{L-1}, B_0..B_{L-1}.  B_i's nonzeros at rows >= rsoe - start[i] read the deeper levels' outputs, which are
+  // still zero when B_i runs (the ascending loop of mod.rs:77-80), so they are dropped here.
+  std::vector<std::vector<uint32_t>> P(2 * L), Cc(2 * L), V(2 * L);
+  for (uint64_t q = 0; q < 2 * L; q++) {
+    const uint64_t i = q % L;
+    const uint64_t *d = q < L ? a_dims + 3 * i : b_dims + 3 * i;
+    const uint64_t lim = q < L ? d[0] : bd->rsoe - bd->start[i];
+    const uint64_t cap = (d[2] && d[0] > UINT64_MAX / d[2]) ? UINT64_MAX : d[0] * d[2];
+    int rc = sprs_pack<R>(d[0], d[1], cap, ind_ptr[q], col_ind[q], val[q], lim, P[q], Cc[q], V[q]);
+    if (rc) return rc;
+  }
+  size_t words = 0;
+  for (uint64_t q = 0; q < 2 * L; q++) words += P[q].size() + Cc[q].size() + V[q].size() + 8;   // +8: keep 32-byte alignment
+  int rc = rt::dev_malloc((void **)&bd->d_mem, words * 4 + 64);
+  if (rc) return rc;
+  rt::stream_t st = ctx->stream;
+  uint32_t *p = bd->d_mem;
+  uint64_t b_first = 0;
+  for (uint64_t q = 0; q < 2 * L; q++) {
+    const uint64_t i = q % L;
+    SprsLevel lv;
+    uint32_t *dv = p;                     // values first: 32-byte aligned loads
+    if (!V[q].empty() && (rc = rt::copy_h2d(dv, V[q].data(), V[q].size() * 4, st))) return rc;
+    p += V[q].size();
+    uint32_t *dp = p;
+    if ((rc = rt::copy_h2d(dp, P[q].data(), P[q].size() * 4, st))) return rc;
+    p += P[q].size();
+    uint32_t *dc = p;
+    if (!Cc[q].empty() && (rc = rt::copy_h2d(dc, Cc[q].data(), Cc[q].size() * 4, st))) return rc;
+    p += Cc[q].size();
+    p += (8 - (size_t)(p - bd->d_mem) % 8) % 8;
+    lv.ind_ptr = dp; lv.col_ind = dc; lv.val = dv;
+    if (q < L) {
+      lv.in_base = bd->start[i] - a_dims[3 * i]; lv.out_base = bd->start[i]; lv.cols = a_dims[3 * i + 1]; lv.first = 0;
+      bd->a_lev.push_back(lv);
+    } else {
+      lv.in_base = bd->start[i]; lv.out_base = bd->end[i]; lv.cols = b_dims[3 * i + 1];
+      bd->b_lev.push_back(lv);
+    }
+  }
+  // the B launch enumerates its output columns from the deepest level (lowest positions) up
+  std::sort(bd->b_lev.begin(), bd->b_lev.end(), [](const SprsLevel &x, const SprsLevel &y) { return x.out_base < y.out_base; });
+  for (SprsLevel &lv : bd->b_lev) { lv.first = b_first; b_first += lv.cols; }
+  return rt::stream_sync(st);
+}
+
+// encode every row of d_in (n_rows x m, row-major) into d_out (n_rows x m_ext, row-major).
+//   work: rsoe * n_rows elements, element-major; rs: (rsie - rss) * n_rows elements
+template <class C>
+static int brakedown_encode_device(const pcgpu_brakedown *bd, const uint32_t *d_in, uint64_t n_rows, uint32_t *work, uint32_t *rs,
+                                   uint32_t *d_out, rt::stream_t st) {
+  using R = typename C::Fr;
+  const uint64_t n = n_rows, m_ext = bd->m_ext;
+  int rc;
+  // cw = msg
+  if ((rc = rt::launch<128>(FrStridedCopyBody{d_in, 1, bd->m, work, n, 1, n}, bd->m * n, st))) return rc;
+  // A levels, each on what the previous one appended
+  for (const SprsLevel &lv : bd->a_lev) {
+    SprsRowMulBody<R> b{};
+    b.lev[0] = lv; b.nlev = 1;
+    b.src = work; b.src_es = n; b.src_rs = 1; b.dst = work; b.dst_es = n; b.dst_rs = 1; b.n_rows = n;
+    if ((rc = rt::launch<128>(b, lv.cols * n, st))) return rc;
+  }
+  // Reed-Solomon in place over cw[rss..rsoe]: its input cw[rss..rsie] is copied aside first
+  const uint64_t n_in = bd->rsie - bd->rss;
+  if ((rc = rt::copy_d2d(rs, work + bd->rss * n * 8, n_in * n * 32, st))) return rc;
+  if ((rc = rt::launch<128>(NaiveRsBody<R>{rs, n_in, work, bd->rss, n}, (bd->rsoe - bd->rss) * n, st))) return rc;
+  // every B level against the buffer as it stands now, straight into the row-major output
+  if (!bd->b_lev.empty()) {
+    SprsRowMulBody<R> b{};
+    for (size_t i = 0; i < bd->b_lev.size(); i++) b.lev[i] = bd->b_lev[i];
+    b.nlev = (uint32_t)bd->b_lev.size();
+    b.src = work; b.src_es = n; b.src_rs = 1; b.dst = d_out; b.dst_es = 1; b.dst_rs = m_ext; b.n_rows = n;
+    if ((rc = rt::launch<128>(b, (m_ext - bd->rsoe) * n, st))) return rc;
+  }
+  // cw[0..rsoe] to the row-major output
+  return rt::launch<128>(FrStridedCopyBody{work, n, 1, d_out, 1, m_ext, n}, bd->rsoe * n, st);
+}
+
+static size_t brakedown_scratch_bytes(const pcgpu_brakedown *bd, uint64_t n_rows) {
+  return rt::Arena::pad(bd->rsoe * n_rows * 32) + rt::Arena::pad((bd->rsie - bd->rss) * n_rows * 32 + 32);
+}
+
+// MultilinearBrakedown::encode over n_rows rows (compute_matrices, linear_codes/mod.rs:118-138) and, when `hash` >= 0, the
+// column hashes and the tree of LinearCodePCS::commit (mod.rs:253-275)
+template <class C>
+int brakedown_commit_impl(pcgpu_ctx *ctx, const pcgpu_brakedown *bd, const void *mat, size_t n_rows, size_t n_cols, int hash,
+                          uint32_t flags, void *out_ext, uint8_t *out_leaves, uint8_t *out_nodes, uint8_t *out_root) {
+  if (n_cols != bd->m) return PCGPU_E_LEN;                   // Error::EncodingError
+  if (n_rows == 0 || n_rows > ((size_t)1 << 40) / bd->m_ext) return PCGPU_E_BADARG;
+  const bool tree = hash >= 0;
+  if (tree && (hash > HASH_SHA256 || bd->m_ext < 2)) return PCGPU_E_BADARG;
+  rt::stream_t st = ctx->stream;
+  const bool dev = (flags & PCGPU_DEVICE_PTRS) != 0;
+  const uint64_t N = bd->m_ext, P = next_pow2_u64(N);
+  size_t need = brakedown_scratch_bytes(bd, n_rows) + 4096;
+  if (!dev) need += rt::Arena::pad(n_rows * n_cols * 32);
+  if (!(dev && out_ext)) need += rt::Arena::pad(n_rows * N * 32);
+  if (tree) need += rt::Arena::pad(N * 32) + rt::Arena::pad((P - 1) * 32);
+  int rc;
+  if ((rc = ctx->stage.reserve(need))) return rc;
+  uint32_t *work = ctx->stage.take<uint32_t>(bd->rsoe * n_rows * 8);
+  uint32_t *rs = ctx->stage.take<uint32_t>((bd->rsie - bd->rss) * n_rows * 8 + 8);
+  uint32_t *d_ext = (dev && out_ext) ? (uint32_t *)out_ext : ctx->stage.take<uint32_t>(n_rows * N * 8);
+  const uint32_t *d_in = (const uint32_t *)mat;
+  if (!dev) {
+    uint32_t *ti = ctx->stage.take<uint32_t>(n_rows * n_cols * 8);
+    if ((rc = rt::copy_h2d(ti, mat, n_rows * n_cols * 32, st))) return rc;
+    d_in = ti;
+  }
+  ctx->prof.begin(15, st);
+  if ((rc = brakedown_encode_device<C>(bd, d_in, n_rows, work, rs, d_ext, st))) return rc;
+  ctx->prof.end(15, st);
+  uint32_t *d_leaves = nullptr, *d_nodes = nullptr;
+  if (tree) {
+    d_leaves = (dev && out_leaves) ? (uint32_t *)out_leaves : ctx->stage.take<uint32_t>(N * 8);
+    d_nodes = (dev && out_nodes) ? (uint32_t *)out_nodes : ctx->stage.take<uint32_t>((P - 1) * 8);
+    ctx->prof.begin(14, st);
+    if ((rc = hash_columns_device<C>(d_ext, n_rows, N, hash, true, d_leaves, st))) return rc;
+    if ((rc = merkle_build(d_leaves, N, P, d_nodes, st))) return rc;
+    ctx->prof.end(14, st);
+  }
+  if (!dev) {
+    if (out_ext && (rc = rt::copy_d2h(out_ext, d_ext, n_rows * N * 32, st))) return rc;
+    if (tree && out_leaves && (rc = rt::copy_d2h(out_leaves, d_leaves, N * 32, st))) return rc;
+    if (tree && out_nodes && (rc = rt::copy_d2h(out_nodes, d_nodes, (P - 1) * 32, st))) return rc;
+  }
+  if (tree && out_root && (rc = rt::copy_d2h(out_root, d_nodes, 32, st))) return rc;
+  rc = rt::stream_sync(st);
+  ctx->prof.collect();
+  return rc;
+}
+
+// SprsMat::row_mul on `count` vectors (count x n, row-major) -> count x m.  The matrix is host data (checked, then staged);
+// with PCGPU_DEVICE_PTRS v and out are device pointers.
+template <class C>
+int fr_sprs_row_mul_impl(pcgpu_ctx *ctx, size_t n, size_t m, const uint64_t *ind_ptr, const uint64_t *col_ind, const void *val,
+                         const void *v, size_t count, uint32_t flags, void *out) {
+  using R = typename C::Fr;
+  std::vector<uint32_t> P, Cc, V;
+  int rc;
+  if ((rc = sprs_pack<R>(n, m, UINT64_MAX, ind_ptr, col_ind, val, n, P, Cc, V))) return rc;
+  if (m == 0 || count == 0) return PCGPU_OK;
+  rt::stream_t st = ctx->stream;
+  const bool dev = (flags & PCGPU_DEVICE_PTRS) != 0;
+  size_t need = rt::Arena::pad(V.size() * 4 + 32) + rt::Arena::pad(P.size() * 4) + rt::Arena::pad(Cc.size() * 4 + 4) + 4096;
+  if (!dev) need += rt::Arena::pad(count * n * 32 + 32) + rt::Arena::pad(count * m * 32);
+  if ((rc = ctx->stage.reserve(need))) return rc;
+  uint32_t *dv = ctx->stage.take<uint32_t>(V.size() + 8), *dp = ctx->stage.take<uint32_t>(P.size()), *dc = ctx->stage.take<uint32_t>(Cc.size() + 1);
+  if (!V.empty() && (rc = rt::copy_h2d(dv, V.data(), V.size() * 4, st))) return rc;
+  if ((rc = rt::copy_h2d(dp, P.data(), P.size() * 4, st))) return rc;
+  if (!Cc.empty() && (rc = rt::copy_h2d(dc, Cc.data(), Cc.size() * 4, st))) return rc;
+  const uint32_t *d_v = (const uint32_t *)v;
+  uint32_t *d_o = (uint32_t *)out;
+  if (!dev) {
+    uint32_t *t = ctx->stage.take<uint32_t>(count * n * 8 + 8);
+    if (n && (rc = rt::copy_h2d(t, v, count * n * 32, st))) return rc;
+    d_v = t; d_o = ctx->stage.take<uint32_t>(count * m * 8);
+  }
+  SprsRowMulBody<R> b{};
+  b.lev[0] = SprsLevel{dp, dc, dv, 0, 0, m, 0}; b.nlev = 1;
+  b.src = d_v; b.src_es = 1; b.src_rs = n; b.dst = d_o; b.dst_es = 1; b.dst_rs = m; b.n_rows = count;
+  if ((rc = rt::launch<128>(b, m * count, st))) return rc;
+  if (!dev && (rc = rt::copy_d2h(out, d_o, count * m * 32, st))) return rc;
+  return rt::stream_sync(st);
+}
+
+// ---------------------------------------------------------------------------------------------
 // G1 wire formats (wire.cuh)
 // ---------------------------------------------------------------------------------------------
 template <class C>
@@ -1603,7 +1855,13 @@ inline int measure_imad_peak_impl(pcgpu_ctx *ctx, double *ops_per_s) {
   EXT template int ntt_batch_impl<C>(pcgpu_ctx *, const void *, size_t, size_t, uint32_t, uint32_t, void *); \
   EXT template int ntt_pass1_peer_impl<C>(pcgpu_ctx *, uint32_t, uint32_t, size_t, size_t, const void *, size_t, void *const *, uint32_t); \
   EXT template int lincode_hash_columns_impl<C>(pcgpu_ctx *, const void *, size_t, size_t, int, uint32_t, uint8_t *); \
-  EXT template int lincode_commit_impl<C>(pcgpu_ctx *, const void *, size_t, size_t, uint32_t, int, uint32_t, void *, uint8_t *, uint8_t *, uint8_t *);
+  EXT template int lincode_commit_impl<C>(pcgpu_ctx *, const void *, size_t, size_t, uint32_t, int, uint32_t, void *, uint8_t *, uint8_t *, uint8_t *); \
+  EXT template int brakedown_register_impl<C>(pcgpu_ctx *, uint64_t, uint64_t, uint64_t, const uint64_t *, const uint64_t *, \
+                                              const uint64_t *const *, const uint64_t *const *, const void *const *, pcgpu_brakedown *); \
+  EXT template int brakedown_commit_impl<C>(pcgpu_ctx *, const pcgpu_brakedown *, const void *, size_t, size_t, int, uint32_t, void *, \
+                                            uint8_t *, uint8_t *, uint8_t *); \
+  EXT template int fr_sprs_row_mul_impl<C>(pcgpu_ctx *, size_t, size_t, const uint64_t *, const uint64_t *, const void *, const void *, \
+                                           size_t, uint32_t, void *);
 #define PCGPU_INST_IPA(C, EXT)                                                                                             \
   EXT template int ipa_begin_impl<C>(pcgpu_ctx *, const void *, size_t, const void *, size_t, const void *, uint32_t, pcgpu_ipa *); \
   EXT template int ipa_round_lr_impl<C>(pcgpu_ctx *, pcgpu_ctx *, pcgpu_ipa *, const void *, void *, uint8_t *, void *, uint8_t *); \

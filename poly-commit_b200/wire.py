@@ -250,3 +250,78 @@ def verifier_key_deserialize(eng, curve, data, compressed=True, validate=True):
     if d.first is not None:
         raise KeyError_(*d.first)
     return dict(g=(xy[0], bool(inf[0])), gamma_g=(xy[1], bool(inf[1])), h=h, beta_h=beta_h, consumed=off)
+
+
+# ---- BrakedownPCParams (linear_codes/data_structures.rs:12-61), derived CanonicalSerialize -------------------------------
+# Field order of the struct; usize = u64 LE, Vec = u64 length + elements, tuples element by element, SprsMat = n, m, d,
+# ind_ptr, col_ind, val (linear_codes/utils.rs:20-37), Fr = 32 canonical LE bytes, bool = one byte.  The three hash
+# parameters are `()` in the configuration of the reference's tests and benches and contribute no bytes.  Needs no device.
+def _fr_canon_bytes(curve, val):
+    from .params import FR_MODULUS
+    r = FR_MODULUS[curve]
+    rinv = pow(1 << 256, -1, r)
+    out = bytearray()
+    for x in np.asarray(val, dtype=np.uint64).reshape(-1, 4):
+        v = (int(x[0]) | int(x[1]) << 64 | int(x[2]) << 128 | int(x[3]) << 192) * rinv % r
+        out += v.to_bytes(32, "little")
+    return bytes(out)
+
+
+def brakedown_params_serialize(params):
+    curve = params["curve"]
+    q = lambda *v: struct.pack("<%dQ" % len(v), *v)
+    vec = lambda xs: q(len(xs)) + b"".join(q(*x) if isinstance(x, tuple) else q(x) for x in xs)
+    out = bytearray(q(params["sec_param"], *params["alpha"], *params["beta"], *params["rho_inv"], params["base_len"], params["n"],
+                      params["m"], params["m_ext"]))
+    out += vec([tuple(x) for x in params["a_dims"]]) + vec([tuple(x) for x in params["b_dims"]])
+    out += vec(list(params["start"])) + vec(list(params["end"]))
+    for mats, dims in ((params["a_mats"], params["a_dims"]), (params["b_mats"], params["b_dims"])):
+        out += q(len(mats))
+        for (ind_ptr, col_ind, val), (n, m, d) in zip(mats, dims):
+            out += q(n, m, d) + vec([int(x) for x in ind_ptr]) + vec([int(x) for x in col_ind])
+            out += q(len(val)) + _fr_canon_bytes(curve, val)
+    out += bytes([1 if params["check_well_formedness"] else 0])
+    return bytes(out)
+
+
+def brakedown_params_deserialize(curve, data):
+    """inverse of brakedown_params_serialize; ValueError on a truncated buffer, trailing bytes, a bool other than 0 / 1 or a
+    field element >= r"""
+    from .params import FR_MODULUS, fr_mont
+    r = FR_MODULUS[curve]
+    data = bytes(data)
+    pos = [0]
+
+    def take(n):
+        if pos[0] + n > len(data):
+            raise ValueError("truncated BrakedownPCParams")
+        b = data[pos[0]:pos[0] + n]
+        pos[0] += n
+        return b
+
+    u = lambda: struct.unpack("<Q", take(8))[0]
+    vec = lambda k: [tuple(u() for _ in range(k)) if k > 1 else u() for _ in range(u())]
+    p = dict(curve=curve, sec_param=u(), alpha=(u(), u()), beta=(u(), u()), rho_inv=(u(), u()), base_len=u(), n=u(), m=u(), m_ext=u())
+    p["a_dims"], p["b_dims"] = vec(3), vec(3)
+    p["start"], p["end"] = vec(1), vec(1)
+    for key in ("a_mats", "b_mats"):
+        mats = []
+        for _ in range(u()):
+            u(), u(), u()                               # n, m, d: repeated from the dims
+            ind_ptr = np.array(vec(1), dtype=np.uint64)
+            col_ind = np.array(vec(1), dtype=np.uint64)
+            vals = []
+            for _ in range(u()):
+                v = int.from_bytes(take(32), "little")
+                if v >= r:
+                    raise ValueError("field element out of range")
+                vals.append(fr_mont(curve, v))
+            mats.append((ind_ptr, col_ind, np.array(vals, dtype=np.uint64).reshape(-1, 4)))
+        p[key] = mats
+    flag = take(1)[0]
+    if flag > 1:
+        raise ValueError("invalid bool")
+    p["check_well_formedness"] = bool(flag)
+    if pos[0] != len(data):
+        raise ValueError("trailing bytes after BrakedownPCParams")
+    return p
