@@ -366,13 +366,16 @@ int pcgpu_selftest_field(pcgpu_ctx *ctx, int curve, uint64_t seed, size_t n, uin
  * kernel; out[PCGPU_GEOM_SPLIT] = blocks per window: 1, 3 or 6) or _BUCKETS (the bucket pipeline: window bits c, windows W,
  * table groups G (1 = raw bases), batched-affine rounds R, the pair-round kernel's threads T and its divisor tdiv, the one
  * resident wave of that kernel the round count was chosen against, entries = n * W, and the number of buckets reduced by
- * the heavy-bucket kernel, or UINT64_MAX where the pipeline's tail did not report it).  Unused fields are 0. */
+ * the heavy-bucket kernel, or UINT64_MAX where the pipeline's tail did not report it) or _COMB (pcgpu_msm_batch over
+ * PCGPU_SRS_COMB tables: n = the row length, c = the comb window bits, W windows, split = the segment length each row is
+ * cut into, entries = count * segments, the number of accumulate tasks).  A pcgpu_msm_batch without comb tables runs its
+ * rows through pcgpu_msm, so it reports the last row's MSM.  Unused fields are 0. */
 enum {
   PCGPU_GEOM_PATH = 0, PCGPU_GEOM_SPLIT = 1, PCGPU_GEOM_N = 2, PCGPU_GEOM_C = 3, PCGPU_GEOM_W = 4, PCGPU_GEOM_G = 5,
   PCGPU_GEOM_R = 6, PCGPU_GEOM_T = 7, PCGPU_GEOM_TDIV = 8, PCGPU_GEOM_WAVE = 9, PCGPU_GEOM_ENTRIES = 10,
   PCGPU_GEOM_HEAVY = 11, PCGPU_GEOM_FIELDS = 12
 };
-enum { PCGPU_MSM_PATH_NONE = 0, PCGPU_MSM_PATH_SMALL = 1, PCGPU_MSM_PATH_BUCKETS = 2 };
+enum { PCGPU_MSM_PATH_NONE = 0, PCGPU_MSM_PATH_SMALL = 1, PCGPU_MSM_PATH_BUCKETS = 2, PCGPU_MSM_PATH_COMB = 3 };
 int pcgpu_msm_last_geometry(pcgpu_ctx *ctx, uint64_t *out, size_t len);
 /* One field primitive applied elementwise on the device (the same code the kernels use), for testing the field layer
  * against plain integers: which = 0 the base field Fq of `curve`, 1 its scalar field Fr.  a, b, out: host arrays of n

@@ -9,7 +9,7 @@ BLS12_381, BN254, PALLAS = 0, 1, 2
 CURVES = {"bls12_381": BLS12_381, "bn254": BN254, "pallas": PALLAS}
 # pcgpu_msm_last_geometry: field names in the header's PCGPU_GEOM_* order, and the PCGPU_MSM_PATH_* values
 GEOM_FIELDS = ("path", "split", "n", "c", "W", "G", "R", "T", "tdiv", "wave", "entries", "heavy")
-MSM_PATH_NONE, MSM_PATH_SMALL, MSM_PATH_BUCKETS = 0, 1, 2
+MSM_PATH_NONE, MSM_PATH_SMALL, MSM_PATH_BUCKETS, MSM_PATH_COMB = 0, 1, 2, 3
 SCALARS_MONT, DEVICE_PTRS, SRS_PRECOMPUTE, NTT_INVERSE, SRS_COMB, WIRE_COMPRESSED, WIRE_NO_VALIDATE = 1, 2, 4, 8, 16, 32, 64
 E_INVALID = -8
 

@@ -511,6 +511,10 @@ int msm_batch_impl(pcgpu_ctx *ctx, const pcgpu_srs *srs, const void *scalars, si
   g.segs = (uint32_t)((n + g.seg_len - 1) / g.seg_len);
   g.scalar_bits = C::Fr::BITS; g.scalars_mont = mont ? 1 : 0;
   size_t ntasks = count * g.segs;
+  uint64_t *lg = ctx->last_geom;
+  memset(lg, 0, sizeof ctx->last_geom);
+  lg[PCGPU_GEOM_PATH] = PCGPU_MSM_PATH_COMB; lg[PCGPU_GEOM_N] = n; lg[PCGPU_GEOM_C] = g.c; lg[PCGPU_GEOM_W] = g.W;
+  lg[PCGPU_GEOM_SPLIT] = g.seg_len; lg[PCGPU_GEOM_ENTRIES] = ntasks;
   size_t need = rt::Arena::pad(ntasks * sizeof(XYZZ<C>)) + rt::Arena::pad(count * psz) + (dev ? 0 : rt::Arena::pad(count * n * 32)) + 8192;
   if ((rc = ctx->stage.reserve(need))) return rc;
   uint32_t *d_err = ctx->stage.take<uint32_t>(16);
