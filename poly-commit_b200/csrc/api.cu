@@ -14,6 +14,39 @@ static int guarded(F f) {
   catch (...) { return PCGPU_E_CUDA; }
 }
 
+// An entry point on one context: BADARG for a null context or when the argument checks found `bad_args`, else f() under the
+// context's mutex with its device current, inside the guard.
+template <class F>
+static int on_ctx(pcgpu_ctx *ctx, bool bad_args, F f) {
+  return guarded([&]() -> int {
+    if (!ctx || bad_args) return PCGPU_E_BADARG;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    SET_DEVICE(ctx);
+    return f();
+  });
+}
+
+// x || y of one affine point of the curve (Montgomery limbs)
+static size_t affine_bytes(int curve) { return (curve == PCGPU_BLS12_381 ? 6 : 4) * 16; }
+
+static void srs_free(pcgpu_srs *srs) {
+  rt::dev_free(srs->d_tables); rt::dev_free(srs->d_folded); rt::dev_free(srs->d_comb);
+}
+
+static void brakedown_free(pcgpu_brakedown *code) { rt::dev_free(code->d_mem); }
+
+// frees device memory that work queued on the context may still read: waits for its stream first (no context: frees at once)
+template <class F>
+static void release_after_stream(pcgpu_ctx *ctx, F free_buffers) {
+  if (!ctx) { free_buffers(); return; }
+  std::lock_guard<std::mutex> lk(ctx->mu);
+#ifndef PCGPU_EMUL
+  cudaSetDevice(ctx->device);
+  cudaStreamSynchronize(ctx->stream);
+#endif
+  free_buffers();
+}
+
 PCGPU_INSTANTIATE(Bls12381, extern)
 PCGPU_INSTANTIATE(Bn254, extern)
 PCGPU_INSTANTIATE(Pallas, extern)
@@ -101,64 +134,41 @@ extern "C" int pcgpu_set_stream(pcgpu_ctx *ctx, void *cuda_stream) {
 }
 
 extern "C" int pcgpu_profile_enable(pcgpu_ctx *ctx, int enable) {
-  return guarded([&]() -> int {
-  if (!ctx) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  ctx->prof.collect();
-  ctx->prof.on = enable != 0;
-  if (enable) ctx->prof.reset();
-  return PCGPU_OK;
+  return on_ctx(ctx, false, [&]() -> int {
+    ctx->prof.collect();
+    ctx->prof.on = enable != 0;
+    if (enable) ctx->prof.reset();
+    return PCGPU_OK;
   });
 }
 
 extern "C" int pcgpu_profile_get(pcgpu_ctx *ctx, int stage, double *ms, uint64_t *count) {
-  return guarded([&]() -> int {
-  if (!ctx || stage < 0 || stage >= PROF_STAGES) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  ctx->prof.collect();
-  if (ms) *ms = ctx->prof.ms[stage];
-  if (count) *count = ctx->prof.cnt[stage];
-  return PCGPU_OK;
+  return on_ctx(ctx, stage < 0 || stage >= PROF_STAGES, [&]() -> int {
+    ctx->prof.collect();
+    if (ms) *ms = ctx->prof.ms[stage];
+    if (count) *count = ctx->prof.cnt[stage];
+    return PCGPU_OK;
   });
 }
 
 extern "C" int pcgpu_srs_register(pcgpu_ctx *ctx, int curve, const void *bases_xy, const uint8_t *inf, size_t n,
                                   uint32_t flags, pcgpu_srs **out) {
-  return guarded([&]() -> int {
-  if (!ctx || !out || (n && !bases_xy) || n >= (1u << 26)) return PCGPU_E_BADARG;
-  *out = nullptr;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  pcgpu_srs *srs = new (std::nothrow) pcgpu_srs();
-  if (!srs) return PCGPU_E_OOM;
-  srs->curve = curve; srs->n = n; srs->d_tables = nullptr; srs->d_folded = nullptr; srs->c = 0; srs->groups = 1; srs->d_comb = nullptr; srs->comb_c = 0;
-  int rc;
-  switch (curve) {
-    case PCGPU_BLS12_381: rc = srs_register_impl<Bls12381>(ctx, bases_xy, inf, n, flags, srs); break;
-    case PCGPU_BN254: rc = srs_register_impl<Bn254>(ctx, bases_xy, inf, n, flags, srs); break;
-    case PCGPU_PALLAS: rc = srs_register_impl<Pallas>(ctx, bases_xy, inf, n, flags, srs); break;
-    default: rc = PCGPU_E_BADARG;
-  }
-  if (rc) { rt::dev_free(srs->d_tables); rt::dev_free(srs->d_folded); rt::dev_free(srs->d_comb); delete srs; return rc; }
-  *out = srs;
-  return PCGPU_OK;
+  const bool bad_args = !out || (n && !bases_xy) || n >= (1u << 26);
+  if (ctx && !bad_args) *out = nullptr;
+  return on_ctx(ctx, bad_args, [&]() -> int {
+    pcgpu_srs *srs = new (std::nothrow) pcgpu_srs();
+    if (!srs) return PCGPU_E_OOM;
+    srs->curve = curve; srs->n = n; srs->d_tables = nullptr; srs->d_folded = nullptr; srs->c = 0; srs->groups = 1; srs->d_comb = nullptr; srs->comb_c = 0;
+    int rc = [&]() -> int { DISPATCH_CURVE(curve, return srs_register_impl<C>(ctx, bases_xy, inf, n, flags, srs)); }();
+    if (rc) { srs_free(srs); delete srs; return rc; }
+    *out = srs;
+    return PCGPU_OK;
   });
 }
 
 extern "C" void pcgpu_srs_release(pcgpu_ctx *ctx, pcgpu_srs *srs) {
   if (!srs) return;
-  if (ctx) {
-    std::lock_guard<std::mutex> lk(ctx->mu);
-#ifndef PCGPU_EMUL
-    cudaSetDevice(ctx->device);
-    cudaStreamSynchronize(ctx->stream);
-#endif
-    rt::dev_free(srs->d_tables); rt::dev_free(srs->d_folded); rt::dev_free(srs->d_comb);
-  } else {
-    rt::dev_free(srs->d_tables); rt::dev_free(srs->d_folded); rt::dev_free(srs->d_comb);
-  }
+  release_after_stream(ctx, [&] { srs_free(srs); });
   delete srs;
 }
 
@@ -167,123 +177,87 @@ extern "C" int pcgpu_srs_curve(const pcgpu_srs *srs) { return srs ? srs->curve :
 
 extern "C" int pcgpu_msm(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, const void *scalars, size_t n,
                          uint32_t flags, void *out_xy, uint8_t *out_inf) {
-  return guarded([&]() -> int {
-  if (!ctx || !srs || (n && !scalars) || !out_xy) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(srs->curve, return msm_impl<C>(ctx, srs, base_offset, scalars, n, flags, out_xy, out_inf, nullptr));
+  return on_ctx(ctx, !srs || (n && !scalars) || !out_xy, [&]() -> int {
+    DISPATCH_CURVE(srs->curve, return msm_impl<C>(ctx, srs, base_offset, scalars, n, flags, out_xy, out_inf, nullptr));
   });
 }
 
 extern "C" int pcgpu_msm_partial(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, const void *scalars, size_t n,
                                  uint32_t flags, void *out_xyzz) {
-  return guarded([&]() -> int {
-  if (!ctx || !srs || (n && !scalars) || !out_xyzz) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(srs->curve, return msm_impl<C>(ctx, srs, base_offset, scalars, n, flags, nullptr, nullptr, out_xyzz));
+  return on_ctx(ctx, !srs || (n && !scalars) || !out_xyzz, [&]() -> int {
+    DISPATCH_CURVE(srs->curve, return msm_impl<C>(ctx, srs, base_offset, scalars, n, flags, nullptr, nullptr, out_xyzz));
   });
 }
 
 extern "C" int pcgpu_g1_sum_xyzz(pcgpu_ctx *ctx, int curve, const void *xyzz, size_t count, void *out_xy, uint8_t *out_inf) {
-  return guarded([&]() -> int {
-  if (!ctx || (count && !xyzz) || !out_xy) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(curve, return g1_sum_impl<C>(ctx, xyzz, count, out_xy, out_inf));
+  return on_ctx(ctx, (count && !xyzz) || !out_xy, [&]() -> int {
+    DISPATCH_CURVE(curve, return g1_sum_impl<C>(ctx, xyzz, count, out_xy, out_inf));
   });
 }
 
 extern "C" int pcgpu_g1_fixed_base_mul(pcgpu_ctx *ctx, int curve, const void *base_xy, const void *scalars, size_t n,
                                        uint32_t flags, void *out_xy) {
-  return guarded([&]() -> int {
-  if (!ctx || !base_xy || (n && (!scalars || !out_xy))) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(curve, return fixed_base_impl<C>(ctx, base_xy, scalars, n, flags, out_xy));
+  return on_ctx(ctx, !base_xy || (n && (!scalars || !out_xy)), [&]() -> int {
+    DISPATCH_CURVE(curve, return fixed_base_impl<C>(ctx, base_xy, scalars, n, flags, out_xy));
   });
 }
 
 extern "C" int pcgpu_fr_from_mont(pcgpu_ctx *ctx, int curve, const void *in, void *out, size_t n, uint32_t flags) {
-  return guarded([&]() -> int {
-  if (!ctx || (n && (!in || !out))) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(curve, return fr_from_mont_impl<C>(ctx, in, out, n, flags));
+  return on_ctx(ctx, (n && (!in || !out)), [&]() -> int {
+    DISPATCH_CURVE(curve, return fr_from_mont_impl<C>(ctx, in, out, n, flags));
   });
 }
 
 extern "C" int pcgpu_fr_axpy(pcgpu_ctx *ctx, int curve, void *y, const void *c, const void *x, size_t n, uint32_t flags) {
-  return guarded([&]() -> int {
-  if (!ctx || !c || (n && (!y || !x))) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(curve, return fr_axpy_impl<C>(ctx, y, c, x, n, flags));
+  return on_ctx(ctx, !c || (n && (!y || !x)), [&]() -> int {
+    DISPATCH_CURVE(curve, return fr_axpy_impl<C>(ctx, y, c, x, n, flags));
   });
 }
 
 extern "C" int pcgpu_fr_div_linear(pcgpu_ctx *ctx, int curve, const void *p, size_t n, const void *z, void *q, void *rem,
                                    uint32_t flags) {
-  return guarded([&]() -> int {
-  if (!ctx || !z || (n && !p) || (n > 1 && !q)) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(curve, return fr_div_impl<C>(ctx, p, n, z, q, rem, flags));
+  return on_ctx(ctx, !z || (n && !p) || (n > 1 && !q), [&]() -> int {
+    DISPATCH_CURVE(curve, return fr_div_impl<C>(ctx, p, n, z, q, rem, flags));
   });
 }
 
 extern "C" int pcgpu_fr_inner_product(pcgpu_ctx *ctx, int curve, const void *a, const void *b, size_t n, void *out,
                                       uint32_t flags) {
-  return guarded([&]() -> int {
-  if (!ctx || !out || (n && (!a || !b))) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(curve, return fr_ip_impl<C>(ctx, a, b, n, out, flags));
+  return on_ctx(ctx, !out || (n && (!a || !b)), [&]() -> int {
+    DISPATCH_CURVE(curve, return fr_ip_impl<C>(ctx, a, b, n, out, flags));
   });
 }
 
 extern "C" int pcgpu_fr_row_mul(pcgpu_ctx *ctx, int curve, const void *v, const void *m, size_t rows, size_t cols, void *out,
                                 uint32_t flags) {
-  return guarded([&]() -> int {
-  if (!ctx || (cols && !out) || (rows && cols && (!v || !m))) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(curve, return fr_row_mul_impl<C>(ctx, v, m, rows, cols, out, flags));
+  return on_ctx(ctx, (cols && !out) || (rows && cols && (!v || !m)), [&]() -> int {
+    DISPATCH_CURVE(curve, return fr_row_mul_impl<C>(ctx, v, m, rows, cols, out, flags));
   });
 }
 
 extern "C" int pcgpu_kzg_commit(pcgpu_ctx *ctx, const pcgpu_srs *powers_of_g, const void *coeffs, size_t n,
                                 const pcgpu_srs *powers_of_gamma_g, const void *blind, size_t n_blind, uint32_t flags,
                                 void *out_xy, uint8_t *out_inf) {
-  return guarded([&]() -> int {
-  if (!ctx || !powers_of_g || (n && !coeffs) || (n_blind && !blind) || !out_xy) return PCGPU_E_BADARG;
-  if (powers_of_gamma_g && powers_of_gamma_g->curve != powers_of_g->curve) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(powers_of_g->curve,
-                 return kzg_commit_impl<C>(ctx, powers_of_g, coeffs, n, powers_of_gamma_g, blind, n_blind, flags, out_xy, out_inf));
+  return on_ctx(ctx, !powers_of_g || (n && !coeffs) || (n_blind && !blind) || !out_xy ||
+                         (powers_of_gamma_g && powers_of_gamma_g->curve != powers_of_g->curve), [&]() -> int {
+    DISPATCH_CURVE(powers_of_g->curve,
+                   return kzg_commit_impl<C>(ctx, powers_of_g, coeffs, n, powers_of_gamma_g, blind, n_blind, flags, out_xy, out_inf));
   });
 }
 
 extern "C" int pcgpu_kzg_open(pcgpu_ctx *ctx, const pcgpu_srs *powers_of_g, const void *coeffs, size_t n, const void *z,
                               const pcgpu_srs *powers_of_gamma_g, const void *blind, size_t n_blind, uint32_t flags,
                               void *out_w_xy, uint8_t *out_w_inf, void *out_random_v) {
-  return guarded([&]() -> int {
-  if (!ctx || !powers_of_g || !z || (n && !coeffs) || (n_blind && !blind) || !out_w_xy) return PCGPU_E_BADARG;
-  if (powers_of_gamma_g && powers_of_gamma_g->curve != powers_of_g->curve) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(powers_of_g->curve, return kzg_open_impl<C>(ctx, powers_of_g, coeffs, n, z, powers_of_gamma_g, blind,
-                                                             n_blind, flags, out_w_xy, out_w_inf, out_random_v));
+  return on_ctx(ctx, !powers_of_g || !z || (n && !coeffs) || (n_blind && !blind) || !out_w_xy ||
+                         (powers_of_gamma_g && powers_of_gamma_g->curve != powers_of_g->curve), [&]() -> int {
+    DISPATCH_CURVE(powers_of_g->curve, return kzg_open_impl<C>(ctx, powers_of_g, coeffs, n, z, powers_of_gamma_g, blind,
+                                                               n_blind, flags, out_w_xy, out_w_inf, out_random_v));
   });
 }
 
 extern "C" int pcgpu_selftest_field(pcgpu_ctx *ctx, int curve, uint64_t seed, size_t n, uint64_t *mismatches) {
-  return guarded([&]() -> int {
-  if (!ctx || !mismatches) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(curve, return selftest_field_impl<C>(ctx, seed, n, mismatches));
+  return on_ctx(ctx, !mismatches, [&]() -> int {
+    DISPATCH_CURVE(curve, return selftest_field_impl<C>(ctx, seed, n, mismatches));
   });
 }
 
@@ -297,54 +271,37 @@ extern "C" int pcgpu_msm_last_geometry(pcgpu_ctx *ctx, uint64_t *out, size_t len
 }
 
 extern "C" int pcgpu_diag_field_op(pcgpu_ctx *ctx, int curve, int which, int op, const void *a, const void *b, void *out, size_t n) {
-  return guarded([&]() -> int {
-  if (!ctx || (which != 0 && which != 1) || op < 0 || op > 9 || (n && (!a || !b || !out))) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(curve, return diag_field_op_impl<C>(ctx, which, op, a, b, out, n));
+  return on_ctx(ctx, (which != 0 && which != 1) || op < 0 || op > 9 || (n && (!a || !b || !out)), [&]() -> int {
+    DISPATCH_CURVE(curve, return diag_field_op_impl<C>(ctx, which, op, a, b, out, n));
   });
 }
 
 extern "C" uint64_t pcgpu_launch_count(void) { return rt::launch_counter().load(); }
 
 extern "C" int pcgpu_ntt(pcgpu_ctx *ctx, int curve, const void *in, size_t n_in, uint32_t logn, uint32_t flags, void *out) {
-  return guarded([&]() -> int {
-  if (!ctx || !out || (n_in && !in)) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(curve, return ntt_impl<C>(ctx, in, n_in, logn, flags, out));
+  return on_ctx(ctx, !out || (n_in && !in), [&]() -> int {
+    DISPATCH_CURVE(curve, return ntt_impl<C>(ctx, in, n_in, logn, flags, out));
   });
 }
 
 extern "C" int pcgpu_msm_batch(pcgpu_ctx *ctx, const pcgpu_srs *srs, const void *scalars, size_t n, size_t count, uint32_t flags,
                                void *out_xy, uint8_t *out_inf) {
-  return guarded([&]() -> int {
-  if (!ctx || !srs || (n && count && !scalars) || (count && !out_xy)) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(srs->curve, return msm_batch_impl<C>(ctx, srs, scalars, n, count, flags, out_xy, out_inf));
+  return on_ctx(ctx, !srs || (n && count && !scalars) || (count && !out_xy), [&]() -> int {
+    DISPATCH_CURVE(srs->curve, return msm_batch_impl<C>(ctx, srs, scalars, n, count, flags, out_xy, out_inf));
   });
 }
 
 extern "C" int pcgpu_ipa_begin(pcgpu_ctx *ctx, int curve, const void *comm_key_xy, size_t n, const void *coeffs, size_t n_coeffs,
                                const void *point, uint32_t flags, pcgpu_ipa **out) {
-  return guarded([&]() -> int {
-  if (!ctx || !out || !comm_key_xy || !point || n == 0 || (n & (n - 1)) || n_coeffs > n || (n_coeffs && !coeffs)) return PCGPU_E_BADARG;
-  *out = nullptr;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  pcgpu_ipa *st = new (std::nothrow) pcgpu_ipa();
-  if (!st) return PCGPU_E_OOM;
-  int rc;
-  switch (curve) {
-    case PCGPU_BLS12_381: rc = ipa_begin_impl<Bls12381>(ctx, comm_key_xy, n, coeffs, n_coeffs, point, flags, st); break;
-    case PCGPU_BN254: rc = ipa_begin_impl<Bn254>(ctx, comm_key_xy, n, coeffs, n_coeffs, point, flags, st); break;
-    case PCGPU_PALLAS: rc = ipa_begin_impl<Pallas>(ctx, comm_key_xy, n, coeffs, n_coeffs, point, flags, st); break;
-    default: rc = PCGPU_E_BADARG;
-  }
-  if (rc) { if (rc != PCGPU_E_BADARG) ctx->ipa_active = false; delete st; return rc; }
-  *out = st;
-  return PCGPU_OK;
+  const bool bad_args = !out || !comm_key_xy || !point || n == 0 || (n & (n - 1)) || n_coeffs > n || (n_coeffs && !coeffs);
+  if (ctx && !bad_args) *out = nullptr;
+  return on_ctx(ctx, bad_args, [&]() -> int {
+    pcgpu_ipa *st = new (std::nothrow) pcgpu_ipa();
+    if (!st) return PCGPU_E_OOM;
+    int rc = [&]() -> int { DISPATCH_CURVE(curve, return ipa_begin_impl<C>(ctx, comm_key_xy, n, coeffs, n_coeffs, point, flags, st)); }();
+    if (rc) { if (rc != PCGPU_E_BADARG) ctx->ipa_active = false; delete st; return rc; }
+    *out = st;
+    return PCGPU_OK;
   });
 }
 
@@ -363,40 +320,25 @@ extern "C" int pcgpu_ipa_round_lr(pcgpu_ctx *ctx, pcgpu_ipa *st, const void *h_p
 }
 
 extern "C" int pcgpu_ipa_round_fold(pcgpu_ctx *ctx, pcgpu_ipa *st, const void *challenge, const void *challenge_inv) {
-  return guarded([&]() -> int {
-  if (!ctx || !st || !challenge || !challenge_inv) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(st->curve, return ipa_round_fold_impl<C>(ctx, st, challenge, challenge_inv));
+  return on_ctx(ctx, !st || !challenge || !challenge_inv, [&]() -> int {
+    DISPATCH_CURVE(st->curve, return ipa_round_fold_impl<C>(ctx, st, challenge, challenge_inv));
   });
 }
 
 extern "C" size_t pcgpu_ipa_len(const pcgpu_ipa *st) { return st ? st->n : 0; }
 
 extern "C" int pcgpu_ipa_finish(pcgpu_ctx *ctx, pcgpu_ipa *st, void *out_final_key_xy, void *out_c) {
-  return guarded([&]() -> int {
-  if (!ctx || !st) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  int rc;
-  switch (st->curve) {
-    case PCGPU_BLS12_381: rc = ipa_finish_impl<Bls12381>(ctx, st, out_final_key_xy, out_c); break;
-    case PCGPU_BN254: rc = ipa_finish_impl<Bn254>(ctx, st, out_final_key_xy, out_c); break;
-    case PCGPU_PALLAS: rc = ipa_finish_impl<Pallas>(ctx, st, out_final_key_xy, out_c); break;
-    default: rc = PCGPU_E_BADARG;
-  }
-  ctx->ipa_active = false;   // the state's memory belongs to the context's IPA arena and is kept for the next open
-  delete st;
-  return rc;
+  return on_ctx(ctx, !st, [&]() -> int {
+    int rc = [&]() -> int { DISPATCH_CURVE(st->curve, return ipa_finish_impl<C>(ctx, st, out_final_key_xy, out_c)); }();
+    ctx->ipa_active = false;   // the state's memory belongs to the context's IPA arena and is kept for the next open
+    delete st;
+    return rc;
   });
 }
 
 extern "C" int pcgpu_measure_imad_peak(pcgpu_ctx *ctx, double *ops_per_s) {
-  return guarded([&]() -> int {
-  if (!ctx || !ops_per_s) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  return measure_imad_peak_impl(ctx, ops_per_s);
+  return on_ctx(ctx, !ops_per_s, [&]() -> int {
+    return measure_imad_peak_impl(ctx, ops_per_s);
   });
 }
 
@@ -406,17 +348,12 @@ extern "C" int pcgpu_kzg_commit_batch(pcgpu_ctx *ctx, const pcgpu_srs *powers_of
                                       size_t count, uint32_t flags, void *out_xy, uint8_t *out_inf) {
   return guarded([&]() -> int {
   if (!ctx || !powers_of_g || (count && (!coeffs || !n || !out_xy))) return PCGPU_E_BADARG;
-  size_t ways = count < (size_t)PCGPU_BATCH_WAYS ? count : (size_t)PCGPU_BATCH_WAYS;
-  {
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    while (ctx->siblings.size() + 1 < ways) {
-      pcgpu_ctx *s = nullptr;
-      int rc = pcgpu_init(ctx->device, &s);
-      if (rc) return rc;
-      ctx->siblings.push_back(s);
-    }
+  const size_t ways = count < (size_t)PCGPU_BATCH_WAYS ? count : (size_t)PCGPU_BATCH_WAYS;
+  if (ways > 1) {   // way 0 runs on ctx itself
+    int rc = ensure_siblings(ctx, ways - 1);
+    if (rc) return rc;
   }
-  const size_t psz = (powers_of_g->curve == PCGPU_BLS12_381 ? 6 : 4) * 16;
+  const size_t psz = affine_bytes(powers_of_g->curve);
   std::vector<int> rcs(ways, PCGPU_OK);
   auto work = [&](size_t w) {
     pcgpu_ctx *c = w == 0 ? ctx : ctx->siblings[w - 1];
@@ -437,11 +374,8 @@ extern "C" int pcgpu_kzg_commit_batch(pcgpu_ctx *ctx, const pcgpu_srs *powers_of
 
 extern "C" int pcgpu_ipa_check_final_key(pcgpu_ctx *ctx, const pcgpu_srs *comm_key, const void *challenges, uint32_t log_d,
                                          void *out_xy, uint8_t *out_inf) {
-  return guarded([&]() -> int {
-  if (!ctx || !comm_key || (log_d && !challenges) || !out_xy) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(comm_key->curve, return ipa_check_final_key_impl<C>(ctx, comm_key, challenges, log_d, out_xy, out_inf));
+  return on_ctx(ctx, !comm_key || (log_d && !challenges) || !out_xy, [&]() -> int {
+    DISPATCH_CURVE(comm_key->curve, return ipa_check_final_key_impl<C>(ctx, comm_key, challenges, log_d, out_xy, out_inf));
   });
 }
 
@@ -453,11 +387,8 @@ extern "C" int pcgpu_ntt_split(uint32_t logn, uint32_t *m1, uint32_t *m2) {
 
 extern "C" int pcgpu_ntt_pass(pcgpu_ctx *ctx, int curve, uint32_t logn, uint32_t flags, int which, size_t lo, size_t count,
                               const void *in, size_t n_in, void *out) {
-  return guarded([&]() -> int {
-  if (!ctx || !out || (n_in && !in)) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(curve, return ntt_pass_impl<C>(ctx, logn, flags, which, lo, count, in, n_in, out));
+  return on_ctx(ctx, !out || (n_in && !in), [&]() -> int {
+    DISPATCH_CURVE(curve, return ntt_pass_impl<C>(ctx, logn, flags, which, lo, count, in, n_in, out));
   });
 }
 
@@ -473,30 +404,21 @@ extern "C" size_t pcgpu_g1_wire_size(int curve, uint32_t flags) {
 
 extern "C" int pcgpu_g1_serialize(pcgpu_ctx *ctx, int curve, const void *xy, const uint8_t *inf, size_t n, uint32_t flags,
                                   uint8_t *out_bytes) {
-  return guarded([&]() -> int {
-  if (!ctx || (n && (!xy || !out_bytes))) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(curve, return g1_serialize_impl<C>(ctx, xy, inf, n, flags, out_bytes));
+  return on_ctx(ctx, (n && (!xy || !out_bytes)), [&]() -> int {
+    DISPATCH_CURVE(curve, return g1_serialize_impl<C>(ctx, xy, inf, n, flags, out_bytes));
   });
 }
 
 extern "C" int pcgpu_g1_deserialize(pcgpu_ctx *ctx, int curve, const uint8_t *bytes, size_t n, uint32_t flags, void *out_xy,
                                     uint8_t *out_inf, size_t *first_bad, int *reason) {
-  return guarded([&]() -> int {
-  if (!ctx || (n && (!bytes || !out_xy || !out_inf))) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(curve, return g1_deserialize_impl<C>(ctx, bytes, n, flags, out_xy, out_inf, first_bad, reason));
+  return on_ctx(ctx, (n && (!bytes || !out_xy || !out_inf)), [&]() -> int {
+    DISPATCH_CURVE(curve, return g1_deserialize_impl<C>(ctx, bytes, n, flags, out_xy, out_inf, first_bad, reason));
   });
 }
 
 extern "C" int pcgpu_fr_mul(pcgpu_ctx *ctx, int curve, const void *a, const void *b, void *out, size_t n, uint32_t flags) {
-  return guarded([&]() -> int {
-  if (!ctx || (n && (!a || !b || !out))) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(curve, return fr_mul_impl<C>(ctx, a, b, out, n, flags));
+  return on_ctx(ctx, (n && (!a || !b || !out)), [&]() -> int {
+    DISPATCH_CURVE(curve, return fr_mul_impl<C>(ctx, a, b, out, n, flags));
   });
 }
 
@@ -518,21 +440,15 @@ extern "C" int pcgpu_msm_bases(pcgpu_ctx *ctx, int curve, const void *bases_xy, 
 
 extern "C" int pcgpu_ntt_batch(pcgpu_ctx *ctx, int curve, const void *in, size_t n_in, size_t count, uint32_t logn, uint32_t flags,
                                void *out) {
-  return guarded([&]() -> int {
-  if (!ctx || (count && (!out || (n_in && !in)))) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(curve, return ntt_batch_impl<C>(ctx, in, n_in, count, logn, flags, out));
+  return on_ctx(ctx, (count && (!out || (n_in && !in))), [&]() -> int {
+    DISPATCH_CURVE(curve, return ntt_batch_impl<C>(ctx, in, n_in, count, logn, flags, out));
   });
 }
 
 extern "C" int pcgpu_ntt_pass1_peer(pcgpu_ctx *ctx, int curve, uint32_t logn, uint32_t flags, size_t lo, size_t count, const void *in,
                                     size_t n_in, void *const *dst, uint32_t world) {
-  return guarded([&]() -> int {
-  if (!ctx || !dst || (n_in && !in)) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(curve, return ntt_pass1_peer_impl<C>(ctx, logn, flags, lo, count, in, n_in, dst, world));
+  return on_ctx(ctx, !dst || (n_in && !in), [&]() -> int {
+    DISPATCH_CURVE(curve, return ntt_pass1_peer_impl<C>(ctx, logn, flags, lo, count, in, n_in, dst, world));
   });
 }
 
@@ -540,70 +456,58 @@ extern "C" int pcgpu_ntt_pass1_peer(pcgpu_ctx *ctx, int curve, uint32_t logn, ui
 extern "C" size_t pcgpu_peer_window_bytes(void) { return (size_t)PEER_WINDOW_BYTES; }
 
 extern "C" int pcgpu_peer_alloc(pcgpu_ctx *ctx, size_t bytes, void **out_ptr, uint8_t *handle) {
-  return guarded([&]() -> int {
-  if (!ctx || !out_ptr || !handle || bytes == 0) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  void *p = nullptr;
-  int rc = rt::dev_malloc(&p, bytes);
-  if (rc) return rc;
-  memset(handle, 0, PCGPU_IPC_HANDLE_BYTES);
+  return on_ctx(ctx, !out_ptr || !handle || bytes == 0, [&]() -> int {
+    void *p = nullptr;
+    int rc = rt::dev_malloc(&p, bytes);
+    if (rc) return rc;
+    memset(handle, 0, PCGPU_IPC_HANDLE_BYTES);
 #ifndef PCGPU_EMUL
-  if (cudaMemset(p, 0, bytes) != cudaSuccess) { rt::dev_free(p); return PCGPU_E_CUDA; }
-  cudaIpcMemHandle_t h;
-  static_assert(sizeof(h) <= PCGPU_IPC_HANDLE_BYTES, "IPC handle larger than the ABI's handle");
-  if (cudaIpcGetMemHandle(&h, p) != cudaSuccess) { rt::dev_free(p); return PCGPU_E_CUDA; }
-  memcpy(handle, &h, sizeof h);
+    if (cudaMemset(p, 0, bytes) != cudaSuccess) { rt::dev_free(p); return PCGPU_E_CUDA; }
+    cudaIpcMemHandle_t h;
+    static_assert(sizeof(h) <= PCGPU_IPC_HANDLE_BYTES, "IPC handle larger than the ABI's handle");
+    if (cudaIpcGetMemHandle(&h, p) != cudaSuccess) { rt::dev_free(p); return PCGPU_E_CUDA; }
+    memcpy(handle, &h, sizeof h);
 #else
-  memset(p, 0, bytes);
-  memcpy(handle, &p, sizeof p);   // emulation: every "rank" lives in this process
+    memset(p, 0, bytes);
+    memcpy(handle, &p, sizeof p);   // emulation: every "rank" lives in this process
 #endif
-  *out_ptr = p;
-  return PCGPU_OK;
+    *out_ptr = p;
+    return PCGPU_OK;
   });
 }
 
 extern "C" int pcgpu_peer_open(pcgpu_ctx *ctx, const uint8_t *handle, void **out_ptr) {
-  return guarded([&]() -> int {
-  if (!ctx || !handle || !out_ptr) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
+  return on_ctx(ctx, !handle || !out_ptr, [&]() -> int {
 #ifndef PCGPU_EMUL
-  cudaIpcMemHandle_t h;
-  memcpy(&h, handle, sizeof h);
-  void *p = nullptr;
-  if (cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) { cudaGetLastError(); return PCGPU_E_CUDA; }
-  *out_ptr = p;
+    cudaIpcMemHandle_t h;
+    memcpy(&h, handle, sizeof h);
+    void *p = nullptr;
+    if (cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) { cudaGetLastError(); return PCGPU_E_CUDA; }
+    *out_ptr = p;
 #else
-  memcpy(out_ptr, handle, sizeof(void *));
+    memcpy(out_ptr, handle, sizeof(void *));
 #endif
-  return PCGPU_OK;
+    return PCGPU_OK;
   });
 }
 
 extern "C" int pcgpu_peer_close(pcgpu_ctx *ctx, void *mapped) {
-  return guarded([&]() -> int {
-  if (!ctx || !mapped) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
+  return on_ctx(ctx, !mapped, [&]() -> int {
 #ifndef PCGPU_EMUL
-  cudaStreamSynchronize(ctx->stream);
-  if (cudaIpcCloseMemHandle(mapped) != cudaSuccess) return PCGPU_E_CUDA;
+    cudaStreamSynchronize(ctx->stream);
+    if (cudaIpcCloseMemHandle(mapped) != cudaSuccess) return PCGPU_E_CUDA;
 #endif
-  return PCGPU_OK;
+    return PCGPU_OK;
   });
 }
 
 extern "C" int pcgpu_peer_free(pcgpu_ctx *ctx, void *ptr) {
-  return guarded([&]() -> int {
-  if (!ctx || !ptr) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
+  return on_ctx(ctx, !ptr, [&]() -> int {
 #ifndef PCGPU_EMUL
-  cudaStreamSynchronize(ctx->stream);
+    cudaStreamSynchronize(ctx->stream);
 #endif
-  rt::dev_free(ptr);
-  return PCGPU_OK;
+    rt::dev_free(ptr);
+    return PCGPU_OK;
   });
 }
 
@@ -614,77 +518,59 @@ static int peer_args_ok(void *const *win, uint32_t rank, uint32_t world) {
 }
 
 extern "C" int pcgpu_peer_signal(pcgpu_ctx *ctx, void *const *win, uint32_t rank, uint32_t world, uint32_t channel, uint64_t epoch) {
-  return guarded([&]() -> int {
-  if (!ctx || !peer_args_ok(win, rank, world) || channel >= 8) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  PeerSignalBody b;
-  memset(&b, 0, sizeof b);
-  for (uint32_t d = 0; d < world; d++) b.win[d] = (char *)win[d];
-  b.rank = rank; b.world = world; b.flag_off = (uint32_t)PEER_FLAG_OFFSET + 256u * channel; b.epoch = epoch;
-  int rc = rt::launch<32>(b, world, ctx->stream);
-  if (rc) return rc;
-  return rt::stream_sync(ctx->stream);
+  return on_ctx(ctx, !peer_args_ok(win, rank, world) || channel >= 8, [&]() -> int {
+    PeerSignalBody b;
+    memset(&b, 0, sizeof b);
+    for (uint32_t d = 0; d < world; d++) b.win[d] = (char *)win[d];
+    b.rank = rank; b.world = world; b.flag_off = (uint32_t)PEER_FLAG_OFFSET + 256u * channel; b.epoch = epoch;
+    int rc = rt::launch<32>(b, world, ctx->stream);
+    if (rc) return rc;
+    return rt::stream_sync(ctx->stream);
   });
 }
 
 extern "C" int pcgpu_peer_wait(pcgpu_ctx *ctx, void *local_win, uint32_t world, uint32_t channel, uint64_t epoch) {
-  return guarded([&]() -> int {
-  if (!ctx || !local_win || world == 0 || world > (uint32_t)PEER_MAX_WORLD || channel >= 8) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  rt::stream_t st = ctx->stream;
-  uint32_t *d_timeout = (uint32_t *)((char *)ctx->d_slots + SLOT_BYTES * NSLOTS);
-  int rc;
-  if ((rc = rt::dev_memset(d_timeout, 0, 4, st))) return rc;
-  if ((rc = rt::launch<32>(PeerWaitBody{(const char *)local_win, world, (uint32_t)PEER_FLAG_OFFSET + 256u * channel, epoch, PEER_WAIT_CYCLES, d_timeout}, world, st))) return rc;
-  uint32_t t = 0;
-  if ((rc = rt::copy_d2h(&t, d_timeout, 4, st))) return rc;
-  if ((rc = rt::stream_sync(st))) return rc;
-  return t ? PCGPU_E_PEER : PCGPU_OK;
+  return on_ctx(ctx, !local_win || world == 0 || world > (uint32_t)PEER_MAX_WORLD || channel >= 8, [&]() -> int {
+    rt::stream_t st = ctx->stream;
+    uint32_t *d_timeout = (uint32_t *)((char *)ctx->d_slots + SLOT_BYTES * NSLOTS);
+    int rc;
+    if ((rc = rt::dev_memset(d_timeout, 0, 4, st))) return rc;
+    if ((rc = rt::launch<32>(PeerWaitBody{(const char *)local_win, world, (uint32_t)PEER_FLAG_OFFSET + 256u * channel, epoch, PEER_WAIT_CYCLES, d_timeout}, world, st))) return rc;
+    uint32_t t = 0;
+    if ((rc = rt::copy_d2h(&t, d_timeout, 4, st))) return rc;
+    if ((rc = rt::stream_sync(st))) return rc;
+    return t ? PCGPU_E_PEER : PCGPU_OK;
   });
 }
 
 extern "C" int pcgpu_msm_peer(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, const void *scalars, size_t n, uint32_t flags,
                               void *const *win, uint32_t rank, uint32_t world, uint64_t epoch, void *out_xy, uint8_t *out_inf) {
-  return guarded([&]() -> int {
-  if (!ctx || !srs || (n && !scalars) || !out_xy || !peer_args_ok(win, rank, world) || epoch == 0) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(srs->curve, return msm_peer_impl<C>(ctx, srs, base_offset, scalars, n, flags, win, rank, world, epoch, out_xy, out_inf));
+  return on_ctx(ctx, !srs || (n && !scalars) || !out_xy || !peer_args_ok(win, rank, world) || epoch == 0, [&]() -> int {
+    DISPATCH_CURVE(srs->curve, return msm_peer_impl<C>(ctx, srs, base_offset, scalars, n, flags, win, rank, world, epoch, out_xy, out_inf));
   });
 }
 
 // ---- linear-code commitments (hash.cuh) ---------------------------------------------------------------------------------
 extern "C" int pcgpu_lincode_hash_columns(pcgpu_ctx *ctx, int curve, const void *ext_mat, size_t n_rows, size_t n_cols, int hash,
                                           uint32_t flags, uint8_t *out_leaves) {
-  return guarded([&]() -> int {
-  if (!ctx || (n_cols && !out_leaves) || (n_rows && n_cols && !ext_mat)) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(curve, return lincode_hash_columns_impl<C>(ctx, ext_mat, n_rows, n_cols, hash, flags, out_leaves));
+  return on_ctx(ctx, (n_cols && !out_leaves) || (n_rows && n_cols && !ext_mat), [&]() -> int {
+    DISPATCH_CURVE(curve, return lincode_hash_columns_impl<C>(ctx, ext_mat, n_rows, n_cols, hash, flags, out_leaves));
   });
 }
 
 extern "C" int pcgpu_merkle_tree(pcgpu_ctx *ctx, const uint8_t *leaves, size_t n_leaves, uint32_t flags, uint8_t *out_nodes,
                                  uint8_t *out_root) {
-  return guarded([&]() -> int {
-  if (!ctx || !leaves) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  return merkle_tree_impl(ctx, leaves, n_leaves, flags, out_nodes, out_root);
+  return on_ctx(ctx, !leaves, [&]() -> int {
+    return merkle_tree_impl(ctx, leaves, n_leaves, flags, out_nodes, out_root);
   });
 }
 
 extern "C" int pcgpu_lincode_commit(pcgpu_ctx *ctx, int curve, const void *mat, size_t n_rows, size_t n_cols, uint32_t log_ext_cols,
                                     int hash, uint32_t flags, void *out_ext_mat, uint8_t *out_leaves, uint8_t *out_nodes,
                                     uint8_t *out_root) {
-  return guarded([&]() -> int {
-  if (!ctx || (n_rows && n_cols && !mat)) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(curve, return lincode_commit_impl<C>(ctx, mat, n_rows, n_cols, log_ext_cols, hash, flags, out_ext_mat, out_leaves,
-                                                      out_nodes, out_root));
+  return on_ctx(ctx, (n_rows && n_cols && !mat), [&]() -> int {
+    DISPATCH_CURVE(curve, return lincode_commit_impl<C>(ctx, mat, n_rows, n_cols, log_ext_cols, hash, flags, out_ext_mat, out_leaves,
+                                                        out_nodes, out_root));
   });
 }
 
@@ -693,70 +579,45 @@ extern "C" int pcgpu_brakedown_register(pcgpu_ctx *ctx, int curve, size_t m, siz
                                         const uint64_t *b_dims, const uint64_t *const *ind_ptr, const uint64_t *const *col_ind,
                                         const void *const *val, uint32_t flags, pcgpu_brakedown **out) {
   (void)flags;
-  return guarded([&]() -> int {
-  if (!ctx || !out) return PCGPU_E_BADARG;
-  *out = nullptr;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  pcgpu_brakedown *bd = new (std::nothrow) pcgpu_brakedown();
-  if (!bd) return PCGPU_E_OOM;
-  bd->d_mem = nullptr;
-  int rc;
-  switch (curve) {
-    case PCGPU_BLS12_381: rc = brakedown_register_impl<Bls12381>(ctx, m, m_ext, levels, a_dims, b_dims, ind_ptr, col_ind, val, bd); break;
-    case PCGPU_BN254: rc = brakedown_register_impl<Bn254>(ctx, m, m_ext, levels, a_dims, b_dims, ind_ptr, col_ind, val, bd); break;
-    case PCGPU_PALLAS: rc = brakedown_register_impl<Pallas>(ctx, m, m_ext, levels, a_dims, b_dims, ind_ptr, col_ind, val, bd); break;
-    default: rc = PCGPU_E_BADARG;
-  }
-  if (rc) { rt::dev_free(bd->d_mem); delete bd; return rc; }
-  *out = bd;
-  return PCGPU_OK;
+  if (ctx && out) *out = nullptr;
+  return on_ctx(ctx, !out, [&]() -> int {
+    pcgpu_brakedown *bd = new (std::nothrow) pcgpu_brakedown();
+    if (!bd) return PCGPU_E_OOM;
+    bd->d_mem = nullptr;
+    int rc = [&]() -> int {
+      DISPATCH_CURVE(curve, return brakedown_register_impl<C>(ctx, m, m_ext, levels, a_dims, b_dims, ind_ptr, col_ind, val, bd));
+    }();
+    if (rc) { brakedown_free(bd); delete bd; return rc; }
+    *out = bd;
+    return PCGPU_OK;
   });
 }
 
 extern "C" void pcgpu_brakedown_release(pcgpu_ctx *ctx, pcgpu_brakedown *code) {
   if (!code) return;
-  if (ctx) {
-    std::lock_guard<std::mutex> lk(ctx->mu);
-#ifndef PCGPU_EMUL
-    cudaSetDevice(ctx->device);
-    cudaStreamSynchronize(ctx->stream);
-#endif
-    rt::dev_free(code->d_mem);
-  } else {
-    rt::dev_free(code->d_mem);
-  }
+  release_after_stream(ctx, [&] { brakedown_free(code); });
   delete code;
 }
 
 extern "C" int pcgpu_brakedown_encode(pcgpu_ctx *ctx, const pcgpu_brakedown *code, const void *mat, size_t n_rows, size_t n_cols,
                                       uint32_t flags, void *out_ext) {
-  return guarded([&]() -> int {
-  if (!ctx || !code || !out_ext || (n_rows && n_cols && !mat)) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(code->curve, return brakedown_commit_impl<C>(ctx, code, mat, n_rows, n_cols, -1, flags, out_ext, nullptr, nullptr, nullptr));
+  return on_ctx(ctx, !code || !out_ext || (n_rows && n_cols && !mat), [&]() -> int {
+    DISPATCH_CURVE(code->curve, return brakedown_commit_impl<C>(ctx, code, mat, n_rows, n_cols, -1, flags, out_ext, nullptr, nullptr, nullptr));
   });
 }
 
 extern "C" int pcgpu_brakedown_commit(pcgpu_ctx *ctx, const pcgpu_brakedown *code, const void *mat, size_t n_rows, size_t n_cols, int hash,
                                       uint32_t flags, void *out_ext, uint8_t *out_leaves, uint8_t *out_nodes, uint8_t *out_root) {
-  return guarded([&]() -> int {
-  if (!ctx || !code || hash < 0 || (n_rows && n_cols && !mat)) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(code->curve, return brakedown_commit_impl<C>(ctx, code, mat, n_rows, n_cols, hash, flags, out_ext, out_leaves, out_nodes,
-                                                              out_root));
+  return on_ctx(ctx, !code || hash < 0 || (n_rows && n_cols && !mat), [&]() -> int {
+    DISPATCH_CURVE(code->curve, return brakedown_commit_impl<C>(ctx, code, mat, n_rows, n_cols, hash, flags, out_ext, out_leaves, out_nodes,
+                                                                out_root));
   });
 }
 
 extern "C" int pcgpu_fr_sprs_row_mul(pcgpu_ctx *ctx, int curve, size_t n, size_t m, const uint64_t *ind_ptr, const uint64_t *col_ind,
                                      const void *val, const void *v, size_t count, uint32_t flags, void *out) {
-  return guarded([&]() -> int {
-  if (!ctx || !ind_ptr || (m && count && !out) || (n && count && !v)) return PCGPU_E_BADARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  SET_DEVICE(ctx);
-  DISPATCH_CURVE(curve, return fr_sprs_row_mul_impl<C>(ctx, n, m, ind_ptr, col_ind, val, v, count, flags, out));
+  return on_ctx(ctx, !ind_ptr || (m && count && !out) || (n && count && !v), [&]() -> int {
+    DISPATCH_CURVE(curve, return fr_sprs_row_mul_impl<C>(ctx, n, m, ind_ptr, col_ind, val, v, count, flags, out));
   });
 }
 
@@ -804,7 +665,7 @@ extern "C" int pcgpu_kzg_commit_open_batch(pcgpu_ctx *ctx, const pcgpu_srs *powe
   if (ways == 0) return PCGPU_OK;
   int rc = ensure_siblings(ctx, 2 * ways - 1);   // way 0: (ctx, sib[0]); way w >= 1: (sib[2w-1], sib[2w])
   if (rc) return rc;
-  const size_t psz = (powers_of_g->curve == PCGPU_BLS12_381 ? 6 : 4) * 16;
+  const size_t psz = affine_bytes(powers_of_g->curve);
   int rcs[PCGPU_COMMIT_OPEN_MAX_WAYS] = {PCGPU_OK, PCGPU_OK, PCGPU_OK, PCGPU_OK};
   // throughput mode of the pair rounds while several pipelines are in flight (msm.cuh); PCGPU_BATCH_TDIV overrides
   uint32_t tdiv = ways >= 2 ? PCGPU_BATCH_PAIR_TDIV : 1;
@@ -832,10 +693,7 @@ extern "C" int pcgpu_kzg_commit_open_batch(pcgpu_ctx *ctx, const pcgpu_srs *powe
 
 // ---- device buffers for callers that keep polynomials on the GPU across calls (PCGPU_DEVICE_PTRS arguments) ------------------
 extern "C" int pcgpu_buf_alloc(pcgpu_ctx *ctx, size_t bytes, void **out) {
-  return guarded([&]() -> int {
-    if (!ctx || !out) return PCGPU_E_BADARG;
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    SET_DEVICE(ctx);
+  return on_ctx(ctx, !out, [&]() -> int {
     void *p = nullptr;
     int rc = rt::dev_malloc(&p, bytes);
     if (rc) return rc;
@@ -845,38 +703,26 @@ extern "C" int pcgpu_buf_alloc(pcgpu_ctx *ctx, size_t bytes, void **out) {
   });
 }
 extern "C" int pcgpu_buf_free(pcgpu_ctx *ctx, void *p) {
-  return guarded([&]() -> int {
-    if (!ctx) return PCGPU_E_BADARG;
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    SET_DEVICE(ctx);
+  return on_ctx(ctx, false, [&]() -> int {
     int rc = rt::stream_sync(ctx->stream);
     rt::dev_free(p);
     return rc;
   });
 }
 extern "C" int pcgpu_buf_write(pcgpu_ctx *ctx, void *dst, size_t dst_off, const void *src, size_t bytes) {
-  return guarded([&]() -> int {
-    if (!ctx || (bytes && (!dst || !src))) return PCGPU_E_BADARG;
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    SET_DEVICE(ctx);
+  return on_ctx(ctx, (bytes && (!dst || !src)), [&]() -> int {
     int rc = bytes ? rt::copy_h2d((char *)dst + dst_off, src, bytes, ctx->stream) : PCGPU_OK;
     return rc ? rc : rt::stream_sync(ctx->stream);
   });
 }
 extern "C" int pcgpu_buf_read(pcgpu_ctx *ctx, const void *src, size_t src_off, void *dst, size_t bytes) {
-  return guarded([&]() -> int {
-    if (!ctx || (bytes && (!dst || !src))) return PCGPU_E_BADARG;
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    SET_DEVICE(ctx);
+  return on_ctx(ctx, (bytes && (!dst || !src)), [&]() -> int {
     int rc = bytes ? rt::copy_d2h(dst, (const char *)src + src_off, bytes, ctx->stream) : PCGPU_OK;
     return rc ? rc : rt::stream_sync(ctx->stream);
   });
 }
 extern "C" int pcgpu_buf_zero(pcgpu_ctx *ctx, void *dst, size_t dst_off, size_t bytes) {
-  return guarded([&]() -> int {
-    if (!ctx || (bytes && !dst)) return PCGPU_E_BADARG;
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    SET_DEVICE(ctx);
+  return on_ctx(ctx, (bytes && !dst), [&]() -> int {
     int rc = bytes ? rt::dev_memset((char *)dst + dst_off, 0, bytes, ctx->stream) : PCGPU_OK;
     return rc ? rc : rt::stream_sync(ctx->stream);
   });
@@ -884,10 +730,7 @@ extern "C" int pcgpu_buf_zero(pcgpu_ctx *ctx, void *dst, size_t dst_off, size_t 
 
 extern "C" int pcgpu_g1_sample_generators(pcgpu_ctx *ctx, int curve, const uint8_t *protocol_name, size_t name_len, uint64_t first_index,
                                           size_t n, uint32_t flags, void *out_xy) {
-  return guarded([&]() -> int {
-    if (!ctx || (name_len && !protocol_name) || (n && !out_xy)) return PCGPU_E_BADARG;
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    SET_DEVICE(ctx);
+  return on_ctx(ctx, (name_len && !protocol_name) || (n && !out_xy), [&]() -> int {
     DISPATCH_CURVE(curve, return g1_sample_generators_impl<C>(ctx, protocol_name, name_len, first_index, n, flags, out_xy));
   });
 }

@@ -114,11 +114,68 @@ static const int NSLOTS = 8;
     default: return PCGPU_E_BADARG;                 \
   }
 
+// The operands of one call that pass through the context's staging arena.  Each operand is declared once, by what it is:
+//   in       with PCGPU_DEVICE_PTRS the caller's pointer as is, else an arena buffer filled from the host
+//   host_in  always a host pointer: an arena buffer filled from it
+//   out      with PCGPU_DEVICE_PTRS and a non-null destination the caller's pointer, else an arena buffer, copied back when
+//            the flag is clear and the destination is non-null
+//   inout    in and out over one buffer
+//   scratch  an arena buffer
+// upload() reserves the arena once from the declared sizes, points every operand at its buffer and queues the host-to-device
+// copies; download() queues the copies back.  Copies go on the context's stream in declaration order; nothing synchronises.
+// Every arena buffer is at least one 256-byte granule, so a zero-length operand still gets a valid, distinct pointer; zero-byte
+// copies are skipped.
+class Staging {
+ public:
+  Staging(pcgpu_ctx *ctx, uint32_t flags) : ctx_(ctx), dev_((flags & PCGPU_DEVICE_PTRS) != 0) {}
+  template <class P> void in(P &d, const void *src, size_t bytes) { add(d, dev_, src, nullptr, bytes, TO_DEV); }
+  template <class P> void host_in(P &d, const void *src, size_t bytes) { add(d, false, src, nullptr, bytes, TO_DEV); }
+  template <class P> void out(P &d, void *dst, size_t bytes) { add(d, dev_ && dst, dst, dev_ ? nullptr : dst, bytes, TO_HOST); }
+  template <class P> void inout(P &d, void *buf, size_t bytes) { add(d, dev_, buf, buf, bytes, TO_DEV | TO_HOST); }
+  template <class P> void scratch(P &d, size_t bytes) { add(d, false, nullptr, nullptr, bytes, 0); }
+  int upload();
+  int download();
 
+ private:
+  enum { TO_DEV = 1, TO_HOST = 2, MAX_OPS = 8 };
+  struct Op { void *slot; void (*set)(void *slot, void *p); const void *src; void *dst; size_t bytes; int copy; void *buf; };
+  template <class P> void add(P &d, bool callers, const void *src, void *dst, size_t bytes, int copy) {
+    if (callers) { d = static_cast<P>(const_cast<void *>(src)); return; }
+    if (n_ == MAX_OPS) { overflow_ = true; return; }
+    ops_[n_++] = Op{&d, [](void *slot, void *p) { *static_cast<P *>(slot) = static_cast<P>(p); }, src, dst, bytes, copy, nullptr};
+  }
+  pcgpu_ctx *ctx_;
+  bool dev_, overflow_ = false;
+  int n_ = 0;
+  Op ops_[MAX_OPS];
+};
 
+inline int Staging::upload() {
+  if (overflow_) return PCGPU_E_BADARG;
+  size_t need = 0;
+  for (int i = 0; i < n_; i++) need += rt::Arena::pad(ops_[i].bytes ? ops_[i].bytes : 1);
+  int rc = ctx_->stage.reserve(need);
+  if (rc) return rc;
+  for (int i = 0; i < n_; i++) {
+    Op &o = ops_[i];
+    if (!(o.buf = ctx_->stage.take<char>(o.bytes ? o.bytes : 1))) return PCGPU_E_OOM;
+    o.set(o.slot, o.buf);
+  }
+  for (int i = 0; i < n_; i++) {
+    const Op &o = ops_[i];
+    if ((o.copy & TO_DEV) && o.bytes && (rc = rt::copy_h2d(o.buf, o.src, o.bytes, ctx_->stream))) return rc;
+  }
+  return PCGPU_OK;
+}
 
-
-
+inline int Staging::download() {
+  int rc;
+  for (int i = 0; i < n_; i++) {
+    const Op &o = ops_[i];
+    if ((o.copy & TO_HOST) && o.dst && o.bytes && (rc = rt::copy_d2h(o.dst, o.buf, o.bytes, ctx_->stream))) return rc;
+  }
+  return PCGPU_OK;
+}
 
 // ---------------------------------------------------------------------------------------------
 // SRS
@@ -164,13 +221,10 @@ int srs_register_impl(pcgpu_ctx *ctx, const void *bases, const uint8_t *inf, siz
     else rc = rt::copy_h2d(srs->d_tables, bases, psz * n, st);
     if (rc) return rc;
     if (inf) {   // identity bases become the device's (0, 0) encoding -- one kernel, for host and device flag arrays alike
-      const uint8_t *d_inf = inf;
-      if (!(flags & PCGPU_DEVICE_PTRS)) {
-        if ((rc = ctx->stage.reserve(rt::Arena::pad(n) + 4096))) return rc;
-        uint8_t *t = ctx->stage.take<uint8_t>(n);
-        if ((rc = rt::copy_h2d(t, inf, n, st))) return rc;
-        d_inf = t;
-      }
+      const uint8_t *d_inf;
+      Staging io(ctx, flags);
+      io.in(d_inf, inf, n);
+      if ((rc = io.upload())) return rc;
       if ((rc = rt::launch<256>(SrsZeroIdentityBody{(uint32_t *)srs->d_tables, d_inf, (uint32_t)(psz / 4)}, n, st))) return rc;
     }
     if (groups > 1 && (rc = srs_build_groups<C>((const Affine<C> *)srs->d_tables, (uint32_t *)srs->d_folded, n, c, groups, st))) return rc;
@@ -365,12 +419,13 @@ int msm_to_host(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, const 
   return msm_collect<C>(ctx, &p, out);
 }
 
-// copies scalars (n x 32 bytes) to the staging arena unless they already live on the device
-static int stage_words(pcgpu_ctx *ctx, const void *src, size_t bytes, uint32_t flags, const uint32_t **out, uint32_t *dst) {
-  if (flags & PCGPU_DEVICE_PTRS) { *out = (const uint32_t *)src; return PCGPU_OK; }
-  int rc = rt::copy_h2d(dst, src, bytes, ctx->stream);
-  *out = dst;
-  return rc;
+// the n scalars (32 bytes each) of an MSM on the device: the caller's (PCGPU_DEVICE_PTRS) or a staged copy
+static int stage_scalars(pcgpu_ctx *ctx, const void *scalars, size_t n, uint32_t flags, const uint32_t **d_scalars) {
+  *d_scalars = nullptr;
+  if (!n) return PCGPU_OK;
+  Staging io(ctx, flags);
+  io.in(*d_scalars, scalars, n * 32);
+  return io.upload();
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -381,14 +436,8 @@ int msm_impl(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, const voi
              void *out_xy, uint8_t *out_inf, void *out_xyzz) {
   if (base_offset > srs->n || n > srs->n - base_offset) return PCGPU_E_LEN;
   int rc;
-  const uint32_t *d_scalars = nullptr;
-  if (n) {
-    if (!(flags & PCGPU_DEVICE_PTRS)) {
-      if ((rc = ctx->stage.reserve(rt::Arena::pad(n * 32) + 4096))) return rc;
-    }
-    uint32_t *buf = (flags & PCGPU_DEVICE_PTRS) ? nullptr : ctx->stage.take<uint32_t>(n * 8);
-    if ((rc = stage_words(ctx, scalars, n * 32, flags, &d_scalars, buf))) return rc;
-  }
+  const uint32_t *d_scalars;
+  if ((rc = stage_scalars(ctx, scalars, n, flags, &d_scalars))) return rc;
   host::HXYZZ<C> r;
   if ((rc = msm_to_host<C>(ctx, srs, base_offset, d_scalars, n, (flags & PCGPU_SCALARS_MONT) != 0, &r))) return rc;
   if (out_xyzz) { memcpy(out_xyzz, &r, sizeof r); return PCGPU_OK; }
@@ -408,14 +457,8 @@ int msm_peer_impl(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, cons
   rt::stream_t st = ctx->stream;
   const bool mont = (flags & PCGPU_SCALARS_MONT) != 0;
   int rc;
-  const uint32_t *d_scalars = nullptr;
-  if (n) {
-    if (!(flags & PCGPU_DEVICE_PTRS)) {
-      if ((rc = ctx->stage.reserve(rt::Arena::pad(n * 32) + 4096))) return rc;
-    }
-    uint32_t *buf = (flags & PCGPU_DEVICE_PTRS) ? nullptr : ctx->stage.take<uint32_t>(n * 8);
-    if ((rc = stage_words(ctx, scalars, n * 32, flags, &d_scalars, buf))) return rc;
-  }
+  const uint32_t *d_scalars;
+  if ((rc = stage_scalars(ctx, scalars, n, flags, &d_scalars))) return rc;
   MsmPeerPushBody push;
   memset(&push, 0, sizeof push);
   for (uint32_t d = 0; d < world; d++) push.win[d] = (char *)win[d];
@@ -494,7 +537,7 @@ int msm_batch_impl(pcgpu_ctx *ctx, const pcgpu_srs *srs, const void *scalars, si
   rt::stream_t st = ctx->stream;
   int rc;
   const size_t psz = sizeof(Affine<C>);
-  bool dev = (flags & PCGPU_DEVICE_PTRS) != 0, mont = (flags & PCGPU_SCALARS_MONT) != 0;
+  const bool mont = (flags & PCGPU_SCALARS_MONT) != 0;
   if (count == 0) return PCGPU_OK;
   if (!srs->d_comb || n == 0) {  // no comb tables: run the rows through the single-MSM pipeline
     for (size_t r = 0; r < count; r++) {
@@ -515,17 +558,13 @@ int msm_batch_impl(pcgpu_ctx *ctx, const pcgpu_srs *srs, const void *scalars, si
   memset(lg, 0, sizeof ctx->last_geom);
   lg[PCGPU_GEOM_PATH] = PCGPU_MSM_PATH_COMB; lg[PCGPU_GEOM_N] = n; lg[PCGPU_GEOM_C] = g.c; lg[PCGPU_GEOM_W] = g.W;
   lg[PCGPU_GEOM_SPLIT] = g.seg_len; lg[PCGPU_GEOM_ENTRIES] = ntasks;
-  size_t need = rt::Arena::pad(ntasks * sizeof(XYZZ<C>)) + rt::Arena::pad(count * psz) + (dev ? 0 : rt::Arena::pad(count * n * 32)) + 8192;
-  if ((rc = ctx->stage.reserve(need))) return rc;
-  uint32_t *d_err = ctx->stage.take<uint32_t>(16);
-  XYZZ<C> *partial = ctx->stage.take<XYZZ<C>>(ntasks);
-  Affine<C> *d_out = ctx->stage.take<Affine<C>>(count);
-  const uint32_t *d_s = (const uint32_t *)scalars;
-  if (!dev) {
-    uint32_t *ts = ctx->stage.take<uint32_t>(count * n * 8);
-    if ((rc = rt::copy_h2d(ts, scalars, count * n * 32, st))) return rc;
-    d_s = ts;
-  }
+  uint32_t *d_err; XYZZ<C> *partial; Affine<C> *d_out; const uint32_t *d_s;
+  Staging io(ctx, flags);
+  io.scratch(d_err, 64);
+  io.scratch(partial, ntasks * sizeof(XYZZ<C>));
+  io.scratch(d_out, count * psz);
+  io.in(d_s, scalars, count * n * 32);
+  if ((rc = io.upload())) return rc;
   if ((rc = rt::dev_memset(d_err, 0, 64, st))) return rc;
   ctx->prof.begin(10, st);
   if ((rc = rt::launch<128>(CombAccumulateBody<C>{(const Affine<C> *)srs->d_comb, d_s, g, partial, d_err}, ntasks, st))) return rc;
@@ -551,21 +590,17 @@ template <class C>
 int fixed_base_impl(pcgpu_ctx *ctx, const void *base_xy, const void *scalars, size_t n, uint32_t flags, void *out_xy) {
   rt::stream_t st = ctx->stream;
   int rc;
-  bool dev = (flags & PCGPU_DEVICE_PTRS) != 0;
-  size_t need = rt::Arena::pad(64 * 15 * sizeof(Affine<C>)) + (dev ? 0 : rt::Arena::pad(n * 32 + 32) + rt::Arena::pad(n * sizeof(Affine<C>) + 32)) + 8192;
-  if ((rc = ctx->stage.reserve(need))) return rc;
-  Affine<C> *table = ctx->stage.take<Affine<C>>(64 * 15);
+  Affine<C> *table, *d_o; const uint32_t *d_s;
+  Staging io(ctx, flags);
+  io.scratch(table, 64 * 15 * sizeof(Affine<C>));
+  io.in(d_s, scalars, n * 32);
+  io.out(d_o, out_xy, n * sizeof(Affine<C>));
+  if ((rc = io.upload())) return rc;
   Affine<C> base;
   memcpy(&base, base_xy, sizeof base);
   if ((rc = rt::launch<64>(FixedBaseTableBody<C>{base, table}, 64, st))) return rc;
-  const uint32_t *d_s = (const uint32_t *)scalars; Affine<C> *d_o = (Affine<C> *)out_xy;
-  if (!dev) {
-    uint32_t *ts = ctx->stage.take<uint32_t>(n * 8 + 8); d_o = ctx->stage.take<Affine<C>>(n + 1);
-    if (n && (rc = rt::copy_h2d(ts, scalars, n * 32, st))) return rc;
-    d_s = ts;
-  }
   if ((rc = rt::launch<128>(FixedBaseMulBody<C>{table, d_s, d_o}, n, st))) return rc;
-  if (!dev && n && (rc = rt::copy_d2h(out_xy, d_o, n * sizeof(Affine<C>), st))) return rc;
+  if ((rc = io.download())) return rc;
   return rt::stream_sync(st);
 }
 
@@ -579,15 +614,13 @@ int fr_from_mont_impl(pcgpu_ctx *ctx, const void *in, void *out, size_t n, uint3
   rt::stream_t st = ctx->stream;
   int rc;
   if (n == 0) return PCGPU_OK;
-  if (flags & PCGPU_DEVICE_PTRS) {
-    if ((rc = rt::launch<256>(FrFromMontBody<R>{(const uint32_t *)in, (uint32_t *)out}, n, st))) return rc;
-    return rt::stream_sync(st);
-  }
-  if ((rc = ctx->stage.reserve(2 * rt::Arena::pad(n * 32) + 4096))) return rc;
-  uint32_t *d_in = ctx->stage.take<uint32_t>(n * 8), *d_out = ctx->stage.take<uint32_t>(n * 8);
-  if ((rc = rt::copy_h2d(d_in, in, n * 32, st))) return rc;
+  const uint32_t *d_in; uint32_t *d_out;
+  Staging io(ctx, flags);
+  io.in(d_in, in, n * 32);
+  io.out(d_out, out, n * 32);
+  if ((rc = io.upload())) return rc;
   if ((rc = rt::launch<256>(FrFromMontBody<R>{d_in, d_out}, n, st))) return rc;
-  if ((rc = rt::copy_d2h(out, d_out, n * 32, st))) return rc;
+  if ((rc = io.download())) return rc;
   return rt::stream_sync(st);
 }
 
@@ -597,16 +630,14 @@ int fr_mul_impl(pcgpu_ctx *ctx, const void *a, const void *b, void *out, size_t 
   rt::stream_t st = ctx->stream;
   int rc;
   if (n == 0) return PCGPU_OK;
-  if (flags & PCGPU_DEVICE_PTRS) {
-    if ((rc = rt::launch<256>(FrMulBody<R>{(const uint32_t *)a, (const uint32_t *)b, (uint32_t *)out}, n, st))) return rc;
-    return rt::stream_sync(st);
-  }
-  if ((rc = ctx->stage.reserve(3 * rt::Arena::pad(n * 32) + 4096))) return rc;
-  uint32_t *d_a = ctx->stage.take<uint32_t>(n * 8), *d_b = ctx->stage.take<uint32_t>(n * 8), *d_o = ctx->stage.take<uint32_t>(n * 8);
-  if ((rc = rt::copy_h2d(d_a, a, n * 32, st))) return rc;
-  if ((rc = rt::copy_h2d(d_b, b, n * 32, st))) return rc;
+  const uint32_t *d_a, *d_b; uint32_t *d_o;
+  Staging io(ctx, flags);
+  io.in(d_a, a, n * 32);
+  io.in(d_b, b, n * 32);
+  io.out(d_o, out, n * 32);
+  if ((rc = io.upload())) return rc;
   if ((rc = rt::launch<256>(FrMulBody<R>{d_a, d_b, d_o}, n, st))) return rc;
-  if ((rc = rt::copy_d2h(out, d_o, n * 32, st))) return rc;
+  if ((rc = io.download())) return rc;
   return rt::stream_sync(st);
 }
 
@@ -616,21 +647,16 @@ int fr_axpy_impl(pcgpu_ctx *ctx, void *y, const void *c, const void *x, size_t n
   rt::stream_t st = ctx->stream;
   int rc;
   if (n == 0) return PCGPU_OK;
-  bool dev = (flags & PCGPU_DEVICE_PTRS) != 0;
-  if ((rc = ctx->stage.reserve((dev ? 0 : 2 * rt::Arena::pad(n * 32)) + 4096))) return rc;
-  uint32_t *d_c = ctx->stage.take<uint32_t>(8);
-  if ((rc = rt::copy_h2d(d_c, c, 32, st))) return rc;
-  uint32_t *d_y = (uint32_t *)y; const uint32_t *d_x = (const uint32_t *)x;
-  if (!dev) {
-    uint32_t *ty = ctx->stage.take<uint32_t>(n * 8), *tx = ctx->stage.take<uint32_t>(n * 8);
-    if ((rc = rt::copy_h2d(ty, y, n * 32, st))) return rc;
-    if ((rc = rt::copy_h2d(tx, x, n * 32, st))) return rc;
-    d_y = ty; d_x = tx;
-  }
+  const uint32_t *d_c, *d_x; uint32_t *d_y;
+  Staging io(ctx, flags);
+  io.host_in(d_c, c, 32);
+  io.inout(d_y, y, n * 32);
+  io.in(d_x, x, n * 32);
+  if ((rc = io.upload())) return rc;
   ctx->prof.begin(8, st);
   if ((rc = rt::launch<256>(FrAxpyBody<R>{d_y, d_c, d_x}, n, st))) return rc;
   ctx->prof.end(8, st);
-  if (!dev && (rc = rt::copy_d2h(y, d_y, n * 32, st))) return rc;
+  if ((rc = io.download())) return rc;
   rc = rt::stream_sync(st);
   ctx->prof.collect();
   return rc;
@@ -642,22 +668,18 @@ int fr_div_impl(pcgpu_ctx *ctx, const void *p, size_t n, const void *z, void *q,
   using R = typename C::Fr;
   rt::stream_t st = ctx->stream;
   int rc;
-  bool dev = (flags & PCGPU_DEVICE_PTRS) != 0;
-  size_t need = rt::Arena::pad(div_scratch_words(n) * 4) + (dev ? 0 : 2 * rt::Arena::pad(n * 32 + 32)) + 8192;
-  if ((rc = ctx->stage.reserve(need))) return rc;
-  uint32_t *d_z = ctx->stage.take<uint32_t>(8), *d_rem = ctx->stage.take<uint32_t>(8);
-  uint32_t *scratch = ctx->stage.take<uint32_t>(div_scratch_words(n));
-  if ((rc = rt::copy_h2d(d_z, z, 32, st))) return rc;
-  const uint32_t *d_p = (const uint32_t *)p; uint32_t *d_q = (uint32_t *)q;
-  if (!dev) {
-    uint32_t *tp = ctx->stage.take<uint32_t>(n * 8 + 8); d_q = ctx->stage.take<uint32_t>(n * 8 + 8);
-    if (n && (rc = rt::copy_h2d(tp, p, n * 32, st))) return rc;
-    d_p = tp;
-  }
+  const uint32_t *d_z, *d_p; uint32_t *d_rem, *scratch, *d_q;
+  Staging io(ctx, flags);
+  io.host_in(d_z, z, 32);
+  io.scratch(d_rem, 32);
+  io.scratch(scratch, div_scratch_words(n) * 4);
+  io.in(d_p, p, n * 32);
+  io.out(d_q, q, n > 1 ? (n - 1) * 32 : 0);
+  if ((rc = io.upload())) return rc;
   ctx->prof.begin(7, st);
   if ((rc = fr_div_linear<R>(d_p, n, d_z, d_q, d_rem, scratch, st))) return rc;
   ctx->prof.end(7, st);
-  if (!dev && n > 1 && (rc = rt::copy_d2h(q, d_q, (n - 1) * 32, st))) return rc;
+  if ((rc = io.download())) return rc;
   uint32_t hrem[8];
   if ((rc = rt::copy_d2h(hrem, d_rem, 32, st))) return rc;
   if ((rc = rt::stream_sync(st))) return rc;
@@ -673,16 +695,13 @@ int fr_ip_impl(pcgpu_ctx *ctx, const void *a, const void *b, size_t n, void *out
   using R = typename C::Fr;
   rt::stream_t st = ctx->stream;
   int rc;
-  bool dev = (flags & PCGPU_DEVICE_PTRS) != 0;
-  if ((rc = ctx->stage.reserve((dev ? 0 : 2 * rt::Arena::pad(n * 32 + 32)) + rt::Arena::pad((IP_THREADS + IP_THREADS / IP_BLOCK + 8) * 32) + 8192))) return rc;
-  uint32_t *scratch = ctx->stage.take<uint32_t>((IP_THREADS + IP_THREADS / IP_BLOCK + 8) * 8), *d_out = ctx->stage.take<uint32_t>(8);
-  const uint32_t *d_a = (const uint32_t *)a, *d_b = (const uint32_t *)b;
-  if (!dev) {
-    uint32_t *ta = ctx->stage.take<uint32_t>(n * 8 + 8), *tb = ctx->stage.take<uint32_t>(n * 8 + 8);
-    if (n && (rc = rt::copy_h2d(ta, a, n * 32, st))) return rc;
-    if (n && (rc = rt::copy_h2d(tb, b, n * 32, st))) return rc;
-    d_a = ta; d_b = tb;
-  }
+  uint32_t *scratch, *d_out; const uint32_t *d_a, *d_b;
+  Staging io(ctx, flags);
+  io.scratch(scratch, (IP_THREADS + IP_THREADS / IP_BLOCK + 8) * 32);
+  io.scratch(d_out, 32);
+  io.in(d_a, a, n * 32);
+  io.in(d_b, b, n * 32);
+  if ((rc = io.upload())) return rc;
   if ((rc = fr_inner_product<R>(d_a, d_b, n, d_out, scratch, st))) return rc;
   if ((rc = rt::copy_d2h(out, d_out, 32, st))) return rc;
   return rt::stream_sync(st);
@@ -694,19 +713,15 @@ int fr_row_mul_impl(pcgpu_ctx *ctx, const void *v, const void *m, size_t rows, s
   using R = typename C::Fr;
   rt::stream_t st = ctx->stream;
   int rc;
-  bool dev = (flags & PCGPU_DEVICE_PTRS) != 0;
   if (cols == 0) return PCGPU_OK;
-  if (dev) {
-    if ((rc = rt::launch<128>(FrRowMulBody<R>{(const uint32_t *)v, (const uint32_t *)m, rows, cols, (uint32_t *)out}, cols, st))) return rc;
-    return rt::stream_sync(st);
-  }
-  if ((rc = ctx->stage.reserve(rt::Arena::pad(rows * 32 + 32) + rt::Arena::pad(rows * cols * 32 + 32) + rt::Arena::pad(cols * 32) + 8192))) return rc;
-  uint32_t *dv = ctx->stage.take<uint32_t>(rows * 8 + 8), *dm = ctx->stage.take<uint32_t>(rows * cols * 8 + 8),
-           *dout = ctx->stage.take<uint32_t>(cols * 8);
-  if (rows && (rc = rt::copy_h2d(dv, v, rows * 32, st))) return rc;
-  if (rows && (rc = rt::copy_h2d(dm, m, rows * cols * 32, st))) return rc;
+  const uint32_t *dv, *dm; uint32_t *dout;
+  Staging io(ctx, flags);
+  io.in(dv, v, rows * 32);
+  io.in(dm, m, rows * cols * 32);
+  io.out(dout, out, cols * 32);
+  if ((rc = io.upload())) return rc;
   if ((rc = rt::launch<128>(FrRowMulBody<R>{dv, dm, rows, cols, dout}, cols, st))) return rc;
-  if ((rc = rt::copy_d2h(out, dout, cols * 32, st))) return rc;
+  if ((rc = io.download())) return rc;
   return rt::stream_sync(st);
 }
 
@@ -729,16 +744,12 @@ int kzg_commit_impl(pcgpu_ctx *ctx, const pcgpu_srs *pg, const void *coeffs, siz
   else { int trc; if ((trc = device_trim_trailing_zeros(ctx, coeffs, &n)) || (trc = device_trim_trailing_zeros(ctx, blind, &n_blind))) return trc; }
   if (n > pg->n) return PCGPU_E_DEGREE;                      // check_degree_is_too_large, kzg10/mod.rs:163
   if (n_blind && (!gamma || n_blind > gamma->n)) return PCGPU_E_HIDING;  // check_hiding_bound, :190-193
-  rt::stream_t st = ctx->stream;
   int rc;
-  if ((rc = ctx->stage.reserve(dev ? 4096 : rt::Arena::pad(n * 32 + 32) + rt::Arena::pad(n_blind * 32 + 32) + 4096))) return rc;
-  const uint32_t *d_c = (const uint32_t *)coeffs, *d_b = (const uint32_t *)blind;
-  if (!dev) {
-    uint32_t *tc = ctx->stage.take<uint32_t>(n * 8 + 8), *tb = ctx->stage.take<uint32_t>(n_blind * 8 + 8);
-    if (n && (rc = rt::copy_h2d(tc, coeffs, n * 32, st))) return rc;
-    if (n_blind && (rc = rt::copy_h2d(tb, blind, n_blind * 32, st))) return rc;
-    d_c = tc; d_b = tb;
-  }
+  const uint32_t *d_c, *d_b;
+  Staging io(ctx, flags);
+  io.in(d_c, coeffs, n * 32);
+  io.in(d_b, blind, n_blind * 32);
+  if ((rc = io.upload())) return rc;
   host::HXYZZ<C> comm, rnd;
   if ((rc = msm_to_host<C>(ctx, pg, 0, d_c, n, true, &comm))) return rc;            // :175-178
   if (n_blind) {
@@ -762,20 +773,17 @@ int kzg_open_impl(pcgpu_ctx *ctx, const pcgpu_srs *pg, const void *coeffs, size_
   if (n_blind && (!gamma || n_blind - 1 > gamma->n)) return PCGPU_E_HIDING;
   rt::stream_t st = ctx->stream;
   int rc;
-  size_t need = rt::Arena::pad(div_scratch_words(n > n_blind ? n : n_blind) * 4) + 2 * rt::Arena::pad(n * 32 + 32) +
-                2 * rt::Arena::pad(n_blind * 32 + 32) + 8192;
-  if ((rc = ctx->stage.reserve(need))) return rc;
-  uint32_t *d_z = ctx->stage.take<uint32_t>(8), *d_rem = ctx->stage.take<uint32_t>(8), *d_rv = ctx->stage.take<uint32_t>(8);
-  uint32_t *scratch = ctx->stage.take<uint32_t>(div_scratch_words(n > n_blind ? n : n_blind));
-  uint32_t *d_q = ctx->stage.take<uint32_t>(n * 8 + 8), *d_bq = ctx->stage.take<uint32_t>(n_blind * 8 + 8);
-  if ((rc = rt::copy_h2d(d_z, z, 32, st))) return rc;
-  const uint32_t *d_c = (const uint32_t *)coeffs, *d_b = (const uint32_t *)blind;
-  if (!dev) {
-    uint32_t *tc = ctx->stage.take<uint32_t>(n * 8 + 8), *tb = ctx->stage.take<uint32_t>(n_blind * 8 + 8);
-    if (n && (rc = rt::copy_h2d(tc, coeffs, n * 32, st))) return rc;
-    if (n_blind && (rc = rt::copy_h2d(tb, blind, n_blind * 32, st))) return rc;
-    d_c = tc; d_b = tb;
-  }
+  const uint32_t *d_z, *d_c, *d_b; uint32_t *d_rem, *d_rv, *scratch, *d_q, *d_bq;
+  Staging io(ctx, flags);
+  io.host_in(d_z, z, 32);
+  io.scratch(d_rem, 32);
+  io.scratch(d_rv, 32);
+  io.scratch(scratch, div_scratch_words(n > n_blind ? n : n_blind) * 4);
+  io.scratch(d_q, n * 32);
+  io.scratch(d_bq, n_blind * 32);
+  io.in(d_c, coeffs, n * 32);
+  io.in(d_b, blind, n_blind * 32);
+  if ((rc = io.upload())) return rc;
   // witness = p / (X - z)   (kzg10/mod.rs:222-226)
   ctx->prof.begin(7, st);
   if ((rc = fr_div_linear<R>(d_c, n, d_z, d_q, d_rem, scratch, st))) return rc;
@@ -852,18 +860,14 @@ int kzg_commit_open_impl(pcgpu_ctx *ctx, pcgpu_ctx *sib, const pcgpu_srs *pg, co
   else if ((rc = device_trim_trailing_zeros(ctx, coeffs, &n))) return rc;
   if (n > pg->n) return PCGPU_E_DEGREE;                      // kzg10/mod.rs:163, :292
   rt::stream_t sa = ctx->stream, sb = sib->stream;
-  if ((rc = ctx->stage.reserve(dev ? 4096 : rt::Arena::pad(n * 32 + 32) + 4096))) return rc;
-  if ((rc = sib->stage.reserve(rt::Arena::pad(div_scratch_words(n) * 4) + rt::Arena::pad(n * 32 + 32) + 8192))) return rc;
-  const uint32_t *d_c = (const uint32_t *)coeffs;
-  if (!dev) {
-    uint32_t *tc = ctx->stage.take<uint32_t>(n * 8 + 8);
-    if (n && (rc = rt::copy_h2d(tc, coeffs, n * 32, sa))) return rc;
-    d_c = tc;
-  }
-  uint32_t *d_z = sib->stage.take<uint32_t>(8), *d_rem = sib->stage.take<uint32_t>(8);
-  uint32_t *scratch = sib->stage.take<uint32_t>(div_scratch_words(n));
-  uint32_t *d_q = sib->stage.take<uint32_t>(n * 8 + 8);
-  if ((rc = rt::copy_h2d(d_z, z, 32, sb))) return rc;
+  const uint32_t *d_c, *d_z; uint32_t *d_rem, *scratch, *d_q;
+  Staging a(ctx, flags), b(sib, flags);   // the coefficients on ctx's stream, the witness side on sib's
+  a.in(d_c, coeffs, n * 32);
+  b.host_in(d_z, z, 32);
+  b.scratch(d_rem, 32);
+  b.scratch(scratch, div_scratch_words(n) * 4);
+  b.scratch(d_q, n * 32);
+  if ((rc = a.upload()) || (rc = b.upload())) return rc;
   if (!ctx->ev_ok) { if ((rc = rt::event_create(&ctx->ev_upload))) return rc; ctx->ev_ok = true; }
   if ((rc = rt::event_record(ctx->ev_upload, sa))) return rc;
   if ((rc = rt::stream_wait_event(sb, ctx->ev_upload))) return rc;
@@ -912,7 +916,6 @@ enum { IPA_FOLD_MIN_BLOCKS = PCGPU_IPA_FOLD_MIN_BLOCKS };
 template <class C>
 static int ipa_freeze(pcgpu_ctx *ctx, pcgpu_ipa *st) {
   using R = typename C::Fr;
-  int rc;
   st->frozen_m = st->n;   // d_w (3 * SMALL_MAX_N elements) was carved out of the context's IPA arena by ipa_begin
   return rt::launch<128>(FrFillOneBody<R>{st->d_w}, st->n, ctx->stream);
 }
@@ -1094,9 +1097,11 @@ int ipa_check_final_key_impl(pcgpu_ctx *ctx, const pcgpu_srs *key, const void *c
   if (n > key->n) return PCGPU_E_LEN;
   rt::stream_t st = ctx->stream;
   int rc;
-  if ((rc = ctx->stage.reserve(rt::Arena::pad(n * 32) + rt::Arena::pad((log_d + 1) * 32) + 4096))) return rc;
-  uint32_t *d_ch = ctx->stage.take<uint32_t>((log_d + 1) * 8), *d_co = ctx->stage.take<uint32_t>(n * 8);
-  if (log_d && (rc = rt::copy_h2d(d_ch, challenges, (size_t)log_d * 32, st))) return rc;
+  const uint32_t *d_ch; uint32_t *d_co;
+  Staging io(ctx, 0);
+  io.host_in(d_ch, challenges, (size_t)log_d * 32);
+  io.scratch(d_co, n * 32);
+  if ((rc = io.upload())) return rc;
   if ((rc = rt::launch<256>(FrCheckCoeffsBody<R>{d_ch, log_d, d_co}, n, st))) return rc;
   host::HXYZZ<C> r;
   if ((rc = msm_to_host<C>(ctx, key, 0, d_co, n, true, &r))) return rc;
@@ -1107,6 +1112,19 @@ int ipa_check_final_key_impl(pcgpu_ctx *ctx, const pcgpu_srs *key, const void *c
 // ---------------------------------------------------------------------------------------------
 // NTT
 // ---------------------------------------------------------------------------------------------
+// the context's twiddle tables for (curve, logn, direction), built on first use
+template <class C>
+static int ntt_plan(pcgpu_ctx *ctx, uint32_t logn, int inverse, const NttPlan **plan) {
+  for (const NttPlan &p : ctx->ntt_plans)
+    if (p.curve == C::ID && p.logn == logn && p.inverse == inverse) { *plan = &p; return PCGPU_OK; }
+  NttPlan p;
+  int rc = ntt_build_plan<typename C::Fr>(p, C::ID, logn, inverse, ctx->stream);
+  if (rc) return rc;
+  ctx->ntt_plans.push_back(p);
+  *plan = &ctx->ntt_plans.back();
+  return PCGPU_OK;
+}
+
 template <class C>
 int ntt_impl(pcgpu_ctx *ctx, const void *in, size_t n_in, uint32_t logn, uint32_t flags, void *out) {
   using R = typename C::Fr;
@@ -1115,27 +1133,18 @@ int ntt_impl(pcgpu_ctx *ctx, const void *in, size_t n_in, uint32_t logn, uint32_
   if (n_in > N) return PCGPU_E_LEN;
   rt::stream_t st = ctx->stream;
   int rc, inverse = (flags & PCGPU_NTT_INVERSE) ? 1 : 0;
-  const NttPlan *plan = nullptr;
-  for (const NttPlan &p : ctx->ntt_plans) if (p.curve == C::ID && p.logn == logn && p.inverse == inverse) plan = &p;
-  if (!plan) {
-    NttPlan p;
-    if ((rc = ntt_build_plan<R>(p, C::ID, logn, inverse, st))) return rc;
-    ctx->ntt_plans.push_back(p);
-    plan = &ctx->ntt_plans.back();
-  }
-  bool dev = (flags & PCGPU_DEVICE_PTRS) != 0;
-  if ((rc = ctx->stage.reserve((dev ? 1 : 3) * rt::Arena::pad(N * 32) + 4096))) return rc;
-  uint32_t *tmp = ctx->stage.take<uint32_t>(N * 8);
-  const uint32_t *d_in = (const uint32_t *)in; uint32_t *d_out = (uint32_t *)out;
-  if (!dev) {
-    uint32_t *ti = ctx->stage.take<uint32_t>(N * 8); d_out = ctx->stage.take<uint32_t>(N * 8);
-    if (n_in && (rc = rt::copy_h2d(ti, in, n_in * 32, st))) return rc;
-    d_in = ti;
-  }
+  const NttPlan *plan;
+  if ((rc = ntt_plan<C>(ctx, logn, inverse, &plan))) return rc;
+  uint32_t *tmp, *d_out; const uint32_t *d_in;
+  Staging io(ctx, flags);
+  io.scratch(tmp, N * 32);
+  io.in(d_in, in, n_in * 32);
+  io.out(d_out, out, N * 32);
+  if ((rc = io.upload())) return rc;
   ctx->prof.begin(9, st);
   if ((rc = ntt_run<R>(*plan, d_in, n_in, d_out, tmp, st))) return rc;
   ctx->prof.end(9, st);
-  if (!dev && (rc = rt::copy_d2h(out, d_out, N * 32, st))) return rc;
+  if ((rc = io.download())) return rc;
   rc = rt::stream_sync(st);
   ctx->prof.collect();
   return rc;
@@ -1154,14 +1163,8 @@ int ntt_pass1_peer_impl(pcgpu_ctx *ctx, uint32_t logn, uint32_t flags, size_t lo
   for (uint32_t d = 0; d < world; d++) if (!dst[d]) return PCGPU_E_BADARG;
   rt::stream_t st = ctx->stream;
   int rc, inverse = (flags & PCGPU_NTT_INVERSE) ? 1 : 0;
-  const NttPlan *plan = nullptr;
-  for (const NttPlan &p : ctx->ntt_plans) if (p.curve == C::ID && p.logn == logn && p.inverse == inverse) plan = &p;
-  if (!plan) {
-    NttPlan p;
-    if ((rc = ntt_build_plan<R>(p, C::ID, logn, inverse, st))) return rc;
-    ctx->ntt_plans.push_back(p);
-    plan = &ctx->ntt_plans.back();
-  }
+  const NttPlan *plan;
+  if ((rc = ntt_plan<C>(ctx, logn, inverse, &plan))) return rc;
   if (count && (rc = ntt_run_pass1_peer<R>(*plan, lo, count, (const uint32_t *)in, n_in, (uint32_t *const *)dst, world, st))) return rc;
   return rt::stream_sync(st);
 }
@@ -1176,31 +1179,19 @@ int ntt_batch_impl(pcgpu_ctx *ctx, const void *in, size_t n_in, size_t count, ui
   if (count > ((size_t)1 << 40) / N) return PCGPU_E_BADARG;
   rt::stream_t st = ctx->stream;
   int rc, inverse = (flags & PCGPU_NTT_INVERSE) ? 1 : 0;
-  const NttPlan *plan = nullptr;
-  for (const NttPlan &p : ctx->ntt_plans) if (p.curve == C::ID && p.logn == logn && p.inverse == inverse) plan = &p;
-  if (!plan) {
-    NttPlan p;
-    if ((rc = ntt_build_plan<R>(p, C::ID, logn, inverse, st))) return rc;
-    ctx->ntt_plans.push_back(p);
-    plan = &ctx->ntt_plans.back();
-  }
-  const bool dev = (flags & PCGPU_DEVICE_PTRS) != 0;
-  const bool multi_pass = plan->m2 != 0;   // rows longer than one block pass: scratch for all rows so both passes are single launches
-  if ((rc = ctx->stage.reserve(rt::Arena::pad(N * 32) + (multi_pass ? rt::Arena::pad(count * N * 32) : 0) +
-                               (dev ? 0 : rt::Arena::pad(count * (n_in ? n_in : 1) * 32) + rt::Arena::pad(count * N * 32)) + 4096)))
-    return rc;
-  uint32_t *tmp = ctx->stage.take<uint32_t>(N * 8);
-  uint32_t *tmp_rows = multi_pass ? ctx->stage.take<uint32_t>(count * N * 8) : nullptr;
-  const uint32_t *d_in = (const uint32_t *)in; uint32_t *d_out = (uint32_t *)out;
-  if (!dev) {
-    uint32_t *ti = ctx->stage.take<uint32_t>(count * (n_in ? n_in : 1) * 8); d_out = ctx->stage.take<uint32_t>(count * N * 8);
-    if (n_in && (rc = rt::copy_h2d(ti, in, count * n_in * 32, st))) return rc;
-    d_in = ti;
-  }
+  const NttPlan *plan;
+  if ((rc = ntt_plan<C>(ctx, logn, inverse, &plan))) return rc;
+  uint32_t *tmp, *tmp_rows = nullptr, *d_out; const uint32_t *d_in;
+  Staging io(ctx, flags);
+  io.scratch(tmp, N * 32);
+  if (plan->m2) io.scratch(tmp_rows, count * N * 32);   // rows longer than one block pass: scratch for all rows so both passes are single launches
+  io.in(d_in, in, count * n_in * 32);
+  io.out(d_out, out, count * N * 32);
+  if ((rc = io.upload())) return rc;
   ctx->prof.begin(9, st);
   if ((rc = ntt_run_batch<R>(*plan, d_in, n_in, count, d_out, tmp, st, tmp_rows))) return rc;
   ctx->prof.end(9, st);
-  if (!dev && (rc = rt::copy_d2h(out, d_out, count * N * 32, st))) return rc;
+  if ((rc = io.download())) return rc;
   rc = rt::stream_sync(st);
   ctx->prof.collect();
   return rc;
@@ -1218,14 +1209,8 @@ int ntt_pass_impl(pcgpu_ctx *ctx, uint32_t logn, uint32_t flags, int which, size
   if (lo > lim || count > lim - lo) return PCGPU_E_LEN;
   rt::stream_t st = ctx->stream;
   int rc, inverse = (flags & PCGPU_NTT_INVERSE) ? 1 : 0;
-  const NttPlan *plan = nullptr;
-  for (const NttPlan &p : ctx->ntt_plans) if (p.curve == C::ID && p.logn == logn && p.inverse == inverse) plan = &p;
-  if (!plan) {
-    NttPlan p;
-    if ((rc = ntt_build_plan<R>(p, C::ID, logn, inverse, st))) return rc;
-    ctx->ntt_plans.push_back(p);
-    plan = &ctx->ntt_plans.back();
-  }
+  const NttPlan *plan;
+  if ((rc = ntt_plan<C>(ctx, logn, inverse, &plan))) return rc;
   if (count && (rc = ntt_run_pass<R>(*plan, which, lo, count, (const uint32_t *)in, n_in, (uint32_t *)out, st))) return rc;
   return rt::stream_sync(st);
 }
@@ -1246,37 +1231,30 @@ static int hash_columns_device(const uint32_t *d_mat, size_t n_rows, size_t n_co
 template <class C>
 int lincode_hash_columns_impl(pcgpu_ctx *ctx, const void *mat, size_t n_rows, size_t n_cols, int hash, uint32_t flags, uint8_t *out_leaves) {
   rt::stream_t st = ctx->stream;
-  const bool dev = (flags & PCGPU_DEVICE_PTRS) != 0;
   int rc;
   if (n_cols == 0) return PCGPU_OK;
-  if (dev) {
-    if ((rc = hash_columns_device<C>((const uint32_t *)mat, n_rows, n_cols, hash, true, (uint32_t *)out_leaves, st))) return rc;
-    return rt::stream_sync(st);
-  }
-  if ((rc = ctx->stage.reserve(rt::Arena::pad(n_rows * n_cols * 32 + 32) + rt::Arena::pad(n_cols * 32) + 4096))) return rc;
-  uint32_t *d_m = ctx->stage.take<uint32_t>(n_rows * n_cols * 8 + 8), *d_l = ctx->stage.take<uint32_t>(n_cols * 8);
-  if (n_rows && (rc = rt::copy_h2d(d_m, mat, n_rows * n_cols * 32, st))) return rc;
+  const uint32_t *d_m; uint32_t *d_l;
+  Staging io(ctx, flags);
+  io.in(d_m, mat, n_rows * n_cols * 32);
+  io.out(d_l, out_leaves, n_cols * 32);
+  if ((rc = io.upload())) return rc;
   if ((rc = hash_columns_device<C>(d_m, n_rows, n_cols, hash, true, d_l, st))) return rc;
-  if ((rc = rt::copy_d2h(out_leaves, d_l, n_cols * 32, st))) return rc;
+  if ((rc = io.download())) return rc;
   return rt::stream_sync(st);
 }
 
 inline int merkle_tree_impl(pcgpu_ctx *ctx, const uint8_t *leaves, size_t n_leaves, uint32_t flags, uint8_t *out_nodes, uint8_t *out_root) {
   rt::stream_t st = ctx->stream;
-  const bool dev = (flags & PCGPU_DEVICE_PTRS) != 0;
   if (n_leaves < 2) return PCGPU_E_BADARG;          // ark-crypto-primitives' MerkleTree::new needs at least two leaves
   const uint64_t P = next_pow2_u64(n_leaves);
   int rc;
-  if ((rc = ctx->stage.reserve((dev ? 0 : rt::Arena::pad(n_leaves * 32)) + rt::Arena::pad((P - 1) * 32) + 4096))) return rc;
-  uint32_t *d_nodes = (dev && out_nodes) ? (uint32_t *)out_nodes : ctx->stage.take<uint32_t>((P - 1) * 8);
-  const uint32_t *d_leaves = (const uint32_t *)leaves;
-  if (!dev) {
-    uint32_t *t = ctx->stage.take<uint32_t>(n_leaves * 8);
-    if ((rc = rt::copy_h2d(t, leaves, n_leaves * 32, st))) return rc;
-    d_leaves = t;
-  }
+  uint32_t *d_nodes; const uint32_t *d_leaves;
+  Staging io(ctx, flags);
+  io.out(d_nodes, out_nodes, (P - 1) * 32);
+  io.in(d_leaves, leaves, n_leaves * 32);
+  if ((rc = io.upload())) return rc;
   if ((rc = merkle_build(d_leaves, n_leaves, P, d_nodes, st))) return rc;
-  if (!dev && out_nodes && (rc = rt::copy_d2h(out_nodes, d_nodes, (P - 1) * 32, st))) return rc;
+  if ((rc = io.download())) return rc;
   if (out_root && (rc = rt::copy_d2h(out_root, d_nodes, 32, st))) return rc;
   return rt::stream_sync(st);
 }
@@ -1292,33 +1270,19 @@ int lincode_commit_impl(pcgpu_ctx *ctx, const void *mat, size_t n_rows, size_t n
   if (N < 2 || n_rows == 0) return PCGPU_E_BADARG;
   if (n_rows > ((size_t)1 << 40) / N) return PCGPU_E_BADARG;
   rt::stream_t st = ctx->stream;
-  const bool dev = (flags & PCGPU_DEVICE_PTRS) != 0;
   int rc;
-  const NttPlan *plan = nullptr;
-  for (const NttPlan &p : ctx->ntt_plans) if (p.curve == C::ID && p.logn == log_ext && p.inverse == 0) plan = &p;
-  if (!plan) {
-    NttPlan p;
-    if ((rc = ntt_build_plan<R>(p, C::ID, log_ext, 0, st))) return rc;
-    ctx->ntt_plans.push_back(p);
-    plan = &ctx->ntt_plans.back();
-  }
+  const NttPlan *plan;
+  if ((rc = ntt_plan<C>(ctx, log_ext, 0, &plan))) return rc;
   const uint64_t P = N;   // the extended width is a power of two already
-  const bool multi_pass = plan->m2 != 0;
-  size_t need = rt::Arena::pad(N * 32) + rt::Arena::pad(N * 32) + rt::Arena::pad((P - 1) * 32) + (multi_pass ? rt::Arena::pad(n_rows * N * 32) : 0) + 4096;
-  if (!dev) need += rt::Arena::pad(n_rows * (n_cols ? n_cols : 1) * 32);
-  if (!(dev && out_ext)) need += rt::Arena::pad(n_rows * N * 32);
-  if ((rc = ctx->stage.reserve(need))) return rc;
-  uint32_t *tmp = ctx->stage.take<uint32_t>(N * 8);
-  uint32_t *tmp_rows = multi_pass ? ctx->stage.take<uint32_t>(n_rows * N * 8) : nullptr;
-  uint32_t *d_leaves = (dev && out_leaves) ? (uint32_t *)out_leaves : ctx->stage.take<uint32_t>(N * 8);
-  uint32_t *d_nodes = (dev && out_nodes) ? (uint32_t *)out_nodes : ctx->stage.take<uint32_t>((P - 1) * 8);
-  uint32_t *d_ext = (dev && out_ext) ? (uint32_t *)out_ext : ctx->stage.take<uint32_t>(n_rows * N * 8);
-  const uint32_t *d_in = (const uint32_t *)mat;
-  if (!dev) {
-    uint32_t *ti = ctx->stage.take<uint32_t>(n_rows * (n_cols ? n_cols : 1) * 8);
-    if (n_cols && (rc = rt::copy_h2d(ti, mat, n_rows * n_cols * 32, st))) return rc;
-    d_in = ti;
-  }
+  uint32_t *tmp, *tmp_rows = nullptr, *d_ext, *d_leaves, *d_nodes; const uint32_t *d_in;
+  Staging io(ctx, flags);
+  io.scratch(tmp, N * 32);
+  if (plan->m2) io.scratch(tmp_rows, n_rows * N * 32);
+  io.out(d_ext, out_ext, n_rows * N * 32);
+  io.out(d_leaves, out_leaves, N * 32);
+  io.out(d_nodes, out_nodes, (P - 1) * 32);
+  io.in(d_in, mat, n_rows * n_cols * 32);
+  if ((rc = io.upload())) return rc;
   ctx->prof.begin(9, st);
   if ((rc = ntt_run_batch<R>(*plan, d_in, n_cols, n_rows, d_ext, tmp, st, tmp_rows))) return rc;
   ctx->prof.end(9, st);
@@ -1326,11 +1290,7 @@ int lincode_commit_impl(pcgpu_ctx *ctx, const void *mat, size_t n_rows, size_t n
   if ((rc = hash_columns_device<C>(d_ext, n_rows, N, hash, true, d_leaves, st))) return rc;
   if ((rc = merkle_build(d_leaves, N, P, d_nodes, st))) return rc;
   ctx->prof.end(14, st);
-  if (!dev) {
-    if (out_ext && (rc = rt::copy_d2h(out_ext, d_ext, n_rows * N * 32, st))) return rc;
-    if (out_leaves && (rc = rt::copy_d2h(out_leaves, d_leaves, N * 32, st))) return rc;
-    if (out_nodes && (rc = rt::copy_d2h(out_nodes, d_nodes, (P - 1) * 32, st))) return rc;
-  }
+  if ((rc = io.download())) return rc;
   if (out_root && (rc = rt::copy_d2h(out_root, d_nodes, 32, st))) return rc;
   rc = rt::stream_sync(st);
   ctx->prof.collect();
@@ -1499,10 +1459,6 @@ static int brakedown_encode_device(const pcgpu_brakedown *bd, const uint32_t *d_
   return rt::launch<128>(FrStridedCopyBody{work, n, 1, d_out, 1, m_ext, n}, bd->rsoe * n, st);
 }
 
-static size_t brakedown_scratch_bytes(const pcgpu_brakedown *bd, uint64_t n_rows) {
-  return rt::Arena::pad(bd->rsoe * n_rows * 32) + rt::Arena::pad((bd->rsie - bd->rss) * n_rows * 32 + 32);
-}
-
 // MultilinearBrakedown::encode over n_rows rows (compute_matrices, linear_codes/mod.rs:118-138) and, when `hash` >= 0, the
 // column hashes and the tree of LinearCodePCS::commit (mod.rs:253-275)
 template <class C>
@@ -1513,40 +1469,30 @@ int brakedown_commit_impl(pcgpu_ctx *ctx, const pcgpu_brakedown *bd, const void 
   const bool tree = hash >= 0;
   if (tree && (hash > HASH_SHA256 || bd->m_ext < 2)) return PCGPU_E_BADARG;
   rt::stream_t st = ctx->stream;
-  const bool dev = (flags & PCGPU_DEVICE_PTRS) != 0;
   const uint64_t N = bd->m_ext, P = next_pow2_u64(N);
-  size_t need = brakedown_scratch_bytes(bd, n_rows) + 4096;
-  if (!dev) need += rt::Arena::pad(n_rows * n_cols * 32);
-  if (!(dev && out_ext)) need += rt::Arena::pad(n_rows * N * 32);
-  if (tree) need += rt::Arena::pad(N * 32) + rt::Arena::pad((P - 1) * 32);
   int rc;
-  if ((rc = ctx->stage.reserve(need))) return rc;
-  uint32_t *work = ctx->stage.take<uint32_t>(bd->rsoe * n_rows * 8);
-  uint32_t *rs = ctx->stage.take<uint32_t>((bd->rsie - bd->rss) * n_rows * 8 + 8);
-  uint32_t *d_ext = (dev && out_ext) ? (uint32_t *)out_ext : ctx->stage.take<uint32_t>(n_rows * N * 8);
-  const uint32_t *d_in = (const uint32_t *)mat;
-  if (!dev) {
-    uint32_t *ti = ctx->stage.take<uint32_t>(n_rows * n_cols * 8);
-    if ((rc = rt::copy_h2d(ti, mat, n_rows * n_cols * 32, st))) return rc;
-    d_in = ti;
+  // work: rsoe * n_rows elements, element-major; rs: (rsie - rss) * n_rows elements (brakedown_encode_device)
+  uint32_t *work, *rs, *d_ext, *d_leaves = nullptr, *d_nodes = nullptr; const uint32_t *d_in;
+  Staging io(ctx, flags);
+  io.scratch(work, bd->rsoe * n_rows * 32);
+  io.scratch(rs, (bd->rsie - bd->rss) * n_rows * 32);
+  io.out(d_ext, out_ext, n_rows * N * 32);
+  if (tree) {
+    io.out(d_leaves, out_leaves, N * 32);
+    io.out(d_nodes, out_nodes, (P - 1) * 32);
   }
+  io.in(d_in, mat, n_rows * n_cols * 32);
+  if ((rc = io.upload())) return rc;
   ctx->prof.begin(15, st);
   if ((rc = brakedown_encode_device<C>(bd, d_in, n_rows, work, rs, d_ext, st))) return rc;
   ctx->prof.end(15, st);
-  uint32_t *d_leaves = nullptr, *d_nodes = nullptr;
   if (tree) {
-    d_leaves = (dev && out_leaves) ? (uint32_t *)out_leaves : ctx->stage.take<uint32_t>(N * 8);
-    d_nodes = (dev && out_nodes) ? (uint32_t *)out_nodes : ctx->stage.take<uint32_t>((P - 1) * 8);
     ctx->prof.begin(14, st);
     if ((rc = hash_columns_device<C>(d_ext, n_rows, N, hash, true, d_leaves, st))) return rc;
     if ((rc = merkle_build(d_leaves, N, P, d_nodes, st))) return rc;
     ctx->prof.end(14, st);
   }
-  if (!dev) {
-    if (out_ext && (rc = rt::copy_d2h(out_ext, d_ext, n_rows * N * 32, st))) return rc;
-    if (tree && out_leaves && (rc = rt::copy_d2h(out_leaves, d_leaves, N * 32, st))) return rc;
-    if (tree && out_nodes && (rc = rt::copy_d2h(out_nodes, d_nodes, (P - 1) * 32, st))) return rc;
-  }
+  if ((rc = io.download())) return rc;
   if (tree && out_root && (rc = rt::copy_d2h(out_root, d_nodes, 32, st))) return rc;
   rc = rt::stream_sync(st);
   ctx->prof.collect();
@@ -1564,26 +1510,19 @@ int fr_sprs_row_mul_impl(pcgpu_ctx *ctx, size_t n, size_t m, const uint64_t *ind
   if ((rc = sprs_pack<R>(n, m, UINT64_MAX, ind_ptr, col_ind, val, n, P, Cc, V))) return rc;
   if (m == 0 || count == 0) return PCGPU_OK;
   rt::stream_t st = ctx->stream;
-  const bool dev = (flags & PCGPU_DEVICE_PTRS) != 0;
-  size_t need = rt::Arena::pad(V.size() * 4 + 32) + rt::Arena::pad(P.size() * 4) + rt::Arena::pad(Cc.size() * 4 + 4) + 4096;
-  if (!dev) need += rt::Arena::pad(count * n * 32 + 32) + rt::Arena::pad(count * m * 32);
-  if ((rc = ctx->stage.reserve(need))) return rc;
-  uint32_t *dv = ctx->stage.take<uint32_t>(V.size() + 8), *dp = ctx->stage.take<uint32_t>(P.size()), *dc = ctx->stage.take<uint32_t>(Cc.size() + 1);
-  if (!V.empty() && (rc = rt::copy_h2d(dv, V.data(), V.size() * 4, st))) return rc;
-  if ((rc = rt::copy_h2d(dp, P.data(), P.size() * 4, st))) return rc;
-  if (!Cc.empty() && (rc = rt::copy_h2d(dc, Cc.data(), Cc.size() * 4, st))) return rc;
-  const uint32_t *d_v = (const uint32_t *)v;
-  uint32_t *d_o = (uint32_t *)out;
-  if (!dev) {
-    uint32_t *t = ctx->stage.take<uint32_t>(count * n * 8 + 8);
-    if (n && (rc = rt::copy_h2d(t, v, count * n * 32, st))) return rc;
-    d_v = t; d_o = ctx->stage.take<uint32_t>(count * m * 8);
-  }
+  const uint32_t *dv, *dp, *dc, *d_v; uint32_t *d_o;
+  Staging io(ctx, flags);
+  io.host_in(dv, V.data(), V.size() * 4);
+  io.host_in(dp, P.data(), P.size() * 4);
+  io.host_in(dc, Cc.data(), Cc.size() * 4);
+  io.in(d_v, v, count * n * 32);
+  io.out(d_o, out, count * m * 32);
+  if ((rc = io.upload())) return rc;
   SprsRowMulBody<R> b{};
   b.lev[0] = SprsLevel{dp, dc, dv, 0, 0, m, 0}; b.nlev = 1;
   b.src = d_v; b.src_es = 1; b.src_rs = n; b.dst = d_o; b.dst_es = 1; b.dst_rs = m; b.n_rows = count;
   if ((rc = rt::launch<128>(b, m * count, st))) return rc;
-  if (!dev && (rc = rt::copy_d2h(out, d_o, count * m * 32, st))) return rc;
+  if ((rc = io.download())) return rc;
   return rt::stream_sync(st);
 }
 
@@ -1598,18 +1537,14 @@ int g1_serialize_impl(pcgpu_ctx *ctx, const void *xy, const uint8_t *inf, size_t
   const size_t sz = wire_size<C>(comp != 0);
   int rc;
   if (n == 0) return PCGPU_OK;
-  if (flags & PCGPU_DEVICE_PTRS) {
-    if ((rc = rt::launch<128>(G1EncodeBody<C>{(const uint32_t *)xy, inf, out, comp}, n, st))) return rc;
-    return rt::stream_sync(st);
-  }
-  if ((rc = ctx->stage.reserve(rt::Arena::pad(n * PT) + rt::Arena::pad(n) + rt::Arena::pad(n * sz) + 4096))) return rc;
-  uint32_t *d_xy = ctx->stage.take<uint32_t>(n * PT / 4);
-  uint8_t *d_inf = inf ? ctx->stage.take<uint8_t>(n) : nullptr;
-  uint8_t *d_out = ctx->stage.take<uint8_t>(n * sz);
-  if ((rc = rt::copy_h2d(d_xy, xy, n * PT, st))) return rc;
-  if (inf && (rc = rt::copy_h2d(d_inf, inf, n, st))) return rc;
+  const uint32_t *d_xy; const uint8_t *d_inf = nullptr; uint8_t *d_out;
+  Staging io(ctx, flags);
+  io.in(d_xy, xy, n * PT);
+  if (inf) io.in(d_inf, inf, n);
+  io.out(d_out, out, n * sz);
+  if ((rc = io.upload())) return rc;
   if ((rc = rt::launch<128>(G1EncodeBody<C>{d_xy, d_inf, d_out, comp}, n, st))) return rc;
-  if ((rc = rt::copy_d2h(out, d_out, n * sz, st))) return rc;
+  if ((rc = io.download())) return rc;
   return rt::stream_sync(st);
 }
 
@@ -1620,29 +1555,19 @@ int g1_deserialize_impl(pcgpu_ctx *ctx, const uint8_t *bytes, size_t n, uint32_t
   rt::stream_t st = ctx->stream;
   const int comp = (flags & PCGPU_WIRE_COMPRESSED) ? 1 : 0, validate = (flags & PCGPU_WIRE_NO_VALIDATE) ? 0 : 1;
   const size_t sz = wire_size<C>(comp != 0);
-  const bool dev = (flags & PCGPU_DEVICE_PTRS) != 0;
   int rc;
   if (n == 0) return PCGPU_OK;
-  if ((rc = ctx->stage.reserve((dev ? 0 : rt::Arena::pad(n * PT) + rt::Arena::pad(n) + rt::Arena::pad(n * sz)) + rt::Arena::pad(n) + 4096)))
-    return rc;
-  uint8_t *d_status = ctx->stage.take<uint8_t>(n);
-  const uint8_t *d_bytes = bytes;
-  uint32_t *d_xy = (uint32_t *)out_xy;
-  uint8_t *d_inf = out_inf;
-  if (!dev) {
-    uint8_t *tb = ctx->stage.take<uint8_t>(n * sz);
-    d_xy = ctx->stage.take<uint32_t>(n * PT / 4);
-    d_inf = ctx->stage.take<uint8_t>(n);
-    if ((rc = rt::copy_h2d(tb, bytes, n * sz, st))) return rc;
-    d_bytes = tb;
-  }
+  uint8_t *d_status, *d_inf; const uint8_t *d_bytes; uint32_t *d_xy;
+  Staging io(ctx, flags);
+  io.scratch(d_status, n);
+  io.in(d_bytes, bytes, n * sz);
+  io.out(d_xy, out_xy, n * PT);
+  io.out(d_inf, out_inf, n);
+  if ((rc = io.upload())) return rc;
   if ((rc = rt::launch<128>(G1DecodeBody<C>{d_bytes, d_xy, d_inf, d_status, comp, validate}, n, st))) return rc;
   std::vector<uint8_t> status(n);
   if ((rc = rt::copy_d2h(status.data(), d_status, n, st))) return rc;
-  if (!dev) {
-    if ((rc = rt::copy_d2h(out_xy, d_xy, n * PT, st))) return rc;
-    if ((rc = rt::copy_d2h(out_inf, d_inf, n, st))) return rc;
-  }
+  if ((rc = io.download())) return rc;
   if ((rc = rt::stream_sync(st))) return rc;
   for (size_t i = 0; i < n; i++)
     if (status[i]) {
@@ -1659,19 +1584,16 @@ int g1_sample_generators_impl(pcgpu_ctx *ctx, const uint8_t *name, size_t name_l
   if (name_len > SAMPLE_NAME_MAX) return PCGPU_E_BADARG;
   if (n == 0) return PCGPU_OK;
   rt::stream_t st = ctx->stream;
-  const bool dev = (flags & PCGPU_DEVICE_PTRS) != 0;
   int rc;
   SampleGeneratorsBody<C> b;
   memset(&b, 0, sizeof b);
   memcpy(b.name, name, name_len);
   b.name_len = (uint32_t)name_len; b.first = first;
-  if (dev) b.out_xy = (uint32_t *)out_xy;
-  else {
-    if ((rc = ctx->stage.reserve(rt::Arena::pad(n * PT) + 4096))) return rc;
-    b.out_xy = ctx->stage.take<uint32_t>(n * PT / 4);
-  }
+  Staging io(ctx, flags);
+  io.out(b.out_xy, out_xy, n * PT);
+  if ((rc = io.upload())) return rc;
   if ((rc = rt::launch<128>(b, n, st))) return rc;
-  if (!dev && (rc = rt::copy_d2h(out_xy, b.out_xy, n * PT, st))) return rc;
+  if ((rc = io.download())) return rc;
   return rt::stream_sync(st);
 }
 
@@ -1716,23 +1638,26 @@ static int diag_field_op_run(pcgpu_ctx *ctx, int op, const void *a, const void *
   rt::stream_t st = ctx->stream;
   const size_t bytes = n * P::N * 4, tbytes = (size_t)(64 * P::N + 1) * P::N * 4;
   int rc;
-  if ((rc = ctx->stage.reserve(3 * rt::Arena::pad(bytes) + rt::Arena::pad(tbytes) + 4096))) return rc;
-  uint32_t *da = ctx->stage.take<uint32_t>(n * P::N), *db = ctx->stage.take<uint32_t>(n * P::N);
-  uint32_t *dout = ctx->stage.take<uint32_t>(n * P::N);
+  const bool fr_table = op == 8 && !std::is_same<P, typename C::Fq>::value;   // no kernel inverts in Fr by binary GCD
+  const uint32_t *da, *db; uint32_t *dout, *t = nullptr;
+  Staging io(ctx, 0);
+  io.host_in(da, a, bytes);
+  io.host_in(db, b, bytes);
+  io.out(dout, out, bytes);
+  if (fr_table) io.scratch(t, tbytes);   // a table for this call only
+  if ((rc = io.upload())) return rc;
   const uint32_t *pow2 = nullptr;
   if (op == 8) {
-    if (std::is_same<P, typename C::Fq>::value) {   // the table the pair rounds use
+    if (!fr_table) {                     // the table the pair rounds use
       if ((rc = ensure_pow2<C>(ctx))) return rc;
       pow2 = ctx->d_pow2[C::ID];
-    } else {                                         // no kernel inverts in Fr by binary GCD: a table for this call only
-      uint32_t *t = ctx->stage.take<uint32_t>(tbytes / 4);
+    } else {
       if ((rc = rt::launch<32>(Pow2TableBody<P>{t}, 1, st))) return rc;
       pow2 = t;
     }
   }
-  if ((rc = rt::copy_h2d(da, a, bytes, st)) || (rc = rt::copy_h2d(db, b, bytes, st))) return rc;
   if ((rc = rt::launch<128>(FieldOpBody<P>{da, db, dout, pow2, op}, n, st))) return rc;
-  if ((rc = rt::copy_d2h(out, dout, bytes, st))) return rc;
+  if ((rc = io.download())) return rc;
   return rt::stream_sync(st);
 }
 
@@ -1796,8 +1721,10 @@ inline int measure_imad_peak_impl(pcgpu_ctx *ctx, double *ops_per_s) {
     return PCGPU_E_CUDA;
   const size_t threads = (size_t)sms * 2048;   // full occupancy: 2048 resident threads per SM
   const uint32_t iters = 4096;
-  if ((rc = ctx->stage.reserve(threads * 8 + 4096))) return rc;
-  uint64_t *sink = ctx->stage.take<uint64_t>(threads);
+  uint64_t *sink;
+  Staging io(ctx, 0);
+  io.scratch(sink, threads * 8);
+  if ((rc = io.upload())) return rc;
   cudaEvent_t e0, e1;
   cudaEventCreate(&e0); cudaEventCreate(&e1);
   if ((rc = rt::launch<256>(ImadPeakBody{sink, 64}, threads, st))) return rc;   // warm-up

@@ -25,8 +25,7 @@ HEAVY_GRID = 64                 # blocks of MsmHeavyBucketBody (grid-strided ove
 DEPTH_SLOTS = 32                # a "depth" case gives every pair-round thread at least this many round-0 slots
 
 
-def on_gpu(eng):
-    return os.path.basename(eng.lib._name) != "libpcgpu_hostcheck.so"
+on_gpu = util.on_gpu
 
 
 def msm_pick_c(n):

@@ -15,7 +15,7 @@ import numpy as np
 import pytest
 
 from oracle import orc, pyref
-from tests import msm_cases, util
+from tests import util
 
 COMB_CHUNK = 256                 # csrc/srs.cuh: table entries one CombTableBody thread builds
 SEG_TASKS = 65536                # csrc/impl.cuh: seg_len halves while a batch has fewer accumulate tasks than this
@@ -93,16 +93,6 @@ def check_rows(cname, bases, canon, got, inf, what):
     tot = orc.g1_sum(C.id, got, inf)
     exp = orc.msm(C.id, bases[:n], colsum)
     assert tot[1] == exp[1] and (tot[0] == exp[0]).all(), (what, "sum of all rows")
-
-
-def dev_ptr(eng, a):
-    """(pointer, owner) of `a` for a DEVICE_PTRS call: the host array under emulation, a CUDA copy on the GPU"""
-    if not msm_cases.on_gpu(eng):
-        return a.ctypes.data, a
-    import torch
-    t = torch.from_numpy(np.ascontiguousarray(a).view(np.int64)).cuda()
-    torch.cuda.synchronize()
-    return t.data_ptr(), t
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
@@ -270,7 +260,7 @@ def error_case(eng, pc, cname, c, monkeypatch, seed=80):
         assert_rows(got, oinf, exp, (cname, "after E_RANGE", hex(bad)))
     mont = orc.field_unop("orc_fr_to_mont", C.id, sc.reshape(-1, 4))
     for arr, flags in ((sc, 0), (mont, pc.SCALARS_MONT)):
-        ptr, keep = dev_ptr(eng, np.ascontiguousarray(arr))
+        ptr, keep = util.dev_ptr(eng, np.ascontiguousarray(arr))
         got, oinf = eng.msm_batch(srs, ptr, n, count, flags=flags | pc.DEVICE_PTRS)
         check_geometry(eng, pc, cname, n, count, c)
         assert_rows(got, oinf, exp, (cname, "device pointers", flags))

@@ -3,7 +3,6 @@ schedule, digit recoding, bucket bookkeeping, scans and the C-ABI host logic, ea
 or the Python big-integer oracle.  These do not replace the GPU parity tests (tests/test_gpu_*.py); they
 catch logic errors before GPU time is spent."""
 import ctypes
-import os
 
 import numpy as np
 import pytest
@@ -20,17 +19,6 @@ def eng(pc, hostcheck_path):
     e = pc.Engine(0, lib_path=hostcheck_path)
     yield e
     e.close()
-
-
-def _dev(eng, a):
-    """(pointer, owner) of `a` for a DEVICE_PTRS call: the host array itself under host emulation, a CUDA copy on the GPU
-    (pageable host memory is not device-accessible in general)"""
-    if os.path.basename(eng.lib._name) == "libpcgpu_hostcheck.so":
-        return a.ctypes.data, a
-    import torch
-    t = torch.from_numpy(np.ascontiguousarray(a).view(np.int64)).cuda()
-    torch.cuda.synchronize()
-    return t.data_ptr(), t
 
 
 def _dev_zeros(eng, shape):
@@ -372,14 +360,14 @@ def test_kzg_commit_open_fused(eng, pc):
     assert ei.value.code == -6
     # "device" pointers (host pointers under emulation): the trailing zeros must be trimmed on the device side as well
     for p, e in zip(polys, exp):
-        dp, _keep = _dev(eng, p)
+        dp, _keep = util.dev_ptr(eng, p)
         (c, ci), (w, wi) = eng.kzg_commit_open(pg, dp, z, n=p.shape[0], flags=pc.DEVICE_PTRS)
         assert (c == e[0]).all() and ci == e[1] and (w == e[2]).all() and wi == e[3]
         got = eng.kzg_commit(pg, dp, n=p.shape[0], flags=pc.DEVICE_PTRS)
         assert (got[0] == e[0]).all() and got[1] == e[1]
     padded = np.zeros((n + 50, 4), dtype=np.uint64)
     padded[:n] = polys[0]
-    dp, _keep = _dev(eng, padded)
+    dp, _keep = util.dev_ptr(eng, padded)
     got = eng.kzg_commit(pg, dp, n=n + 50, flags=pc.DEVICE_PTRS)   # zero-padded beyond the SRS length: no E_DEGREE
     assert (got[0] == exp[0][0]).all()
     got = eng.kzg_open(pg, dp, z, n=n + 50, flags=pc.DEVICE_PTRS)
@@ -1214,7 +1202,7 @@ def test_ntt_pass1_with_fused_exchange(eng, cname, logn, world):
     rows, cols = N1 // world, N2 // world
     n_in = (1 << logn) - 5
     x = util.rand_fr(cname, n_in, seed=200 + logn, mont=True)
-    xp, _keep = _dev(eng, x)
+    xp, _keep = util.dev_ptr(eng, x)
     for inverse in (False, True):
         rowbufs = [_dev_zeros(eng, (rows, N2, 4)) for _ in range(world)]
         ptrs = [p for p, _ in rowbufs]

@@ -1,4 +1,6 @@
 """Shared helpers for the parity tests: seeded synthetic inputs in the ABI's packed layout."""
+import os
+
 import numpy as np
 
 from oracle import orc, pyref
@@ -9,6 +11,22 @@ _SRS_CACHE = {}
 
 def rng(seed):
     return np.random.default_rng(seed)
+
+
+def on_gpu(eng):
+    """True for the CUDA library, False for the host-emulated one (tests/host_emul)"""
+    return os.path.basename(eng.lib._name) != "libpcgpu_hostcheck.so"
+
+
+def dev_ptr(eng, a):
+    """(pointer, owner) of `a` for a DEVICE_PTRS call: the host array itself under host emulation, a CUDA copy on the GPU
+    (pageable host memory is not device-accessible in general)"""
+    if not on_gpu(eng):
+        return a.ctypes.data, a
+    import torch
+    t = torch.from_numpy(np.ascontiguousarray(a).reshape(-1).view(np.uint8)).cuda()
+    torch.cuda.synchronize()
+    return t.data_ptr(), t
 
 
 def rand_fr_ints(curve, n, seed):
