@@ -37,6 +37,11 @@ typedef struct pcgpu_srs pcgpu_srs;
 
 /* curve ids mirror the type parameter E / G of the reference's schemes */
 enum { PCGPU_BLS12_381 = 0, PCGPU_BN254 = 1, PCGPU_PALLAS = 2 };
+/* G2 group ids (E::G2 of the pairing curves): 0x100 + the curve id, out of the range of curve ids.  Accepted where a key's
+ * group is named -- pcgpu_srs_register, pcgpu_msm_bases, pcgpu_g2_fixed_base_mul -- and by pcgpu_msm through the key; every
+ * entry point that takes a scalar-field or G1 curve returns PCGPU_E_BADARG for them.  A G2 affine point is
+ * x.c0 || x.c1 || y.c0 || y.c1, each `limbs` u64 Montgomery (Fq2 = Fq[u] / (u^2 + 1)), plus the separate infinity byte. */
+enum { PCGPU_BLS12_381_G2 = 0x100, PCGPU_BN254_G2 = 0x101 };
 
 enum {
   PCGPU_OK = 0,
@@ -71,14 +76,16 @@ int pcgpu_set_stream(pcgpu_ctx *ctx, void *cuda_stream);
 /* Per-stage device timings (CUDA events on the launching stream).  stage: 0 digits/count, 1 scan,
  * 2 scatter, 3 tasks, 4 bucket accumulate (XYZZ), 5 bucket reduce, 6 final (host tail, wall clock), 7 fr division,
  * 8 fr axpy, 9 ntt, 10 comb batch, 11 affine pair rounds (all), 12 affine pair round 0 kernel alone, 13 peer push + wait,
- * 14 column hashes + Merkle tree, 15 Brakedown encoding.
+ * 14 column hashes + Merkle tree, 15 Brakedown encoding, 16 MultilinearPC open fold chain.
  * enable=1 starts recording; get returns accumulated milliseconds and launch count since enable. */
 int pcgpu_profile_enable(pcgpu_ctx *ctx, int enable);
 int pcgpu_profile_get(pcgpu_ctx *ctx, int stage, double *ms, uint64_t *count);
 
 /* ---- SRS / committer key ---------------------------------------------------------------------- */
 /* Upload n affine bases once (kzg10 Powers::powers_of_g, data_structures.rs:124-129; ipa CommitterKey::comm_key;
- * hyrax com_key).  inf may be NULL (no identity points). */
+ * hyrax com_key).  inf may be NULL (no identity points).  `curve` may be a G2 group id: the key then holds raw G2 bases
+ * (PCGPU_SRS_PRECOMPUTE and PCGPU_SRS_COMB return PCGPU_E_BADARG) and pcgpu_msm over it is
+ * <E::G2 as VariableBaseMSM>::msm_bigint, run without batched-affine rounds. */
 int pcgpu_srs_register(pcgpu_ctx *ctx, int curve, const void *bases_xy, const uint8_t *inf, size_t n, uint32_t flags,
                        pcgpu_srs **out);
 void pcgpu_srs_release(pcgpu_ctx *ctx, pcgpu_srs *srs);
@@ -119,6 +126,10 @@ int pcgpu_msm_bases(pcgpu_ctx *ctx, int curve, const void *bases_xy, const uint8
  * SRSs on the device).  base_xy: one affine point (host).  scalars: n canonical.  out_xy: n affine points, x||y only
  * (an identity result is written as x = y = 0).  With PCGPU_DEVICE_PTRS scalars and out_xy are device pointers. */
 int pcgpu_g1_fixed_base_mul(pcgpu_ctx *ctx, int curve, const void *base_xy, const void *scalars, size_t n, uint32_t flags,
+                            void *out_xy);
+/* The same in G2: h.batch_mul(scalars), MultilinearPC::setup (multilinear_pc/mod.rs:62).  group: PCGPU_BLS12_381_G2 or
+ * PCGPU_BN254_G2; base_xy and out_xy are G2 affine points. */
+int pcgpu_g2_fixed_base_mul(pcgpu_ctx *ctx, int group, const void *base_xy, const void *scalars, size_t n, uint32_t flags,
                             void *out_xy);
 
 /* InnerProductArgPC::sample_generators (ipa_pc/mod.rs:302-325) and HyraxPC::setup's generator loop (hyrax/mod.rs:143-163):
@@ -302,6 +313,26 @@ int pcgpu_ipa_finish(pcgpu_ctx *ctx, pcgpu_ipa *st, void *out_final_key_xy, void
 int pcgpu_ipa_check_final_key(pcgpu_ctx *ctx, const pcgpu_srs *comm_key, const void *challenges, uint32_t log_d,
                               void *out_xy, uint8_t *out_inf);
 
+/* ---- MultilinearPC (XZZPD19, multilinear_pc/mod.rs) prover -----------------------------------------------------------
+ * pcgpu_mlpc_register: the G2 half of a CommitterKey (after trim, :91-111).  curve: PCGPU_BLS12_381 or PCGPU_BN254.  Level i
+ *   = 0 .. nv-1 is powers_of_h[i], 2^(nv-i) G2 affine points, with inf[i] its infinity bytes (inf or inf[i] may be NULL).  The
+ *   key stores the pair-folded bases H'_i[b] = H_i[2b] + H_i[2b+1], one device G2 addition per pair, so that an open runs
+ *   2^nv - 1 G2 terms; this holds for any key, honestly generated or not.  With PCGPU_DEVICE_PTRS the level arrays are
+ *   device pointers.  1 <= nv <= 25.
+ * pcgpu_mlpc_open: MultilinearPC::open (:131-168).  evals: the 2^nv Montgomery Fr values of the polynomial in
+ *   to_evaluations() order (PCGPU_DEVICE_PTRS: a device pointer); point: nv Montgomery Fr (host).  The fold chain
+ *   q_i[b] = r[2b+1] - r[2b], r'[b] = r[2b] (1 - point[i]) + r[2b+1] point[i] runs on the device (profile stage 16), then
+ *   proof i = sum_b q_i[b] H'_i[b].  out_proofs_xy: nv G2 affine points, out_proofs_inf: nv bytes (may be NULL),
+ *   out_value (may be NULL): the last r, which is p(point), Montgomery Fr.  n != 2^nv: PCGPU_E_LEN ("Invalid size of
+ *   polynomial", :136).
+ * The commitment (:114-128) is pcgpu_msm with PCGPU_SCALARS_MONT over a G1 key of powers_of_g[0]. */
+typedef struct pcgpu_mlpc pcgpu_mlpc;
+int pcgpu_mlpc_register(pcgpu_ctx *ctx, int curve, uint32_t nv, const void *const *powers_of_h, const uint8_t *const *inf,
+                        uint32_t flags, pcgpu_mlpc **out);
+void pcgpu_mlpc_release(pcgpu_ctx *ctx, pcgpu_mlpc *key);
+int pcgpu_mlpc_open(pcgpu_ctx *ctx, const pcgpu_mlpc *key, const void *evals, size_t n, const void *point, uint32_t flags,
+                    void *out_proofs_xy, uint8_t *out_proofs_inf, void *out_value);
+
 /* ---- KZG10 fused prover calls ------------------------------------------------------------------ */
 /* KZG10::commit -- kzg10/mod.rs:157-210.  coeffs: n Montgomery Fr (low degree first; trailing zeros allowed and
  * ignored like DensePolynomial's truncation).  Hiding: pass gamma (powers_of_gamma_g) and n_blind > 0 blinding
@@ -378,7 +409,8 @@ enum {
 enum { PCGPU_MSM_PATH_NONE = 0, PCGPU_MSM_PATH_SMALL = 1, PCGPU_MSM_PATH_BUCKETS = 2, PCGPU_MSM_PATH_COMB = 3 };
 int pcgpu_msm_last_geometry(pcgpu_ctx *ctx, uint64_t *out, size_t len);
 /* One field primitive applied elementwise on the device (the same code the kernels use), for testing the field layer
- * against plain integers: which = 0 the base field Fq of `curve`, 1 its scalar field Fr.  a, b, out: host arrays of n
+ * against plain integers: which = 0 the base field Fq of `curve`, 1 its scalar field Fr, 2 its quadratic extension Fq2
+ * (pairing curves only; elements c0 || c1; ops 0, 2, 3, 4, 5 (through the norm) and 9 (a^2)).  a, b, out: host arrays of n
  * elements, little-endian 32-bit limbs (Fq of BLS12-381: 12 limbs, every other field 8), Montgomery form.  op:
  *   0 mont_mul(a, b)   1 mont_mul_ref(a, b) (plain 64-bit accumulate)   2 a + b   3 a - b   4 -a   5 a^-1 (Fermat)
  *   6 mont_mul2(a, b, b, -a) (= 0)   7 mont_mul2(a, b, a + b, b - a)   8 a^-1 (binary GCD)   9 mont_sqr(a)

@@ -7,6 +7,9 @@ import numpy as np
 
 BLS12_381, BN254, PALLAS = 0, 1, 2
 CURVES = {"bls12_381": BLS12_381, "bn254": BN254, "pallas": PALLAS}
+# G2 group ids of the pairing curves (include/pcgpu.h): keys, MSMs and fixed-base multiplications in E::G2
+BLS12_381_G2, BN254_G2 = 0x100, 0x101
+G2_OF = {BLS12_381: BLS12_381_G2, BN254: BN254_G2}
 # pcgpu_msm_last_geometry: field names in the header's PCGPU_GEOM_* order, and the PCGPU_MSM_PATH_* values
 GEOM_FIELDS = ("path", "split", "n", "c", "W", "G", "R", "T", "tdiv", "wave", "entries", "heavy")
 MSM_PATH_NONE, MSM_PATH_SMALL, MSM_PATH_BUCKETS, MSM_PATH_COMB = 0, 1, 2, 3
@@ -18,6 +21,13 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 
 def fq_limbs(curve):
     return 6 if curve == BLS12_381 else 4
+
+
+def affine_limbs(group):
+    """u64 words of one affine point of a group id: x||y in G1, x.c0||x.c1||y.c0||y.c1 in G2"""
+    if group in (BLS12_381_G2, BN254_G2):
+        return 4 * fq_limbs(group & 0xFF)
+    return 2 * fq_limbs(group)
 
 
 def library_path():
@@ -75,6 +85,11 @@ def _load(path):
         "pcgpu_msm_partial": [_vp, _vp, _sz, _vp, _sz, ctypes.c_uint32, _vp],
         "pcgpu_g1_sum_xyzz": [_vp, ctypes.c_int, _vp, _sz, _vp, _vp],
         "pcgpu_g1_fixed_base_mul": [_vp, ctypes.c_int, _vp, _vp, _sz, ctypes.c_uint32, _vp],
+        "pcgpu_g2_fixed_base_mul": [_vp, ctypes.c_int, _vp, _vp, _sz, ctypes.c_uint32, _vp],
+        "pcgpu_mlpc_register": [_vp, ctypes.c_int, ctypes.c_uint32, ctypes.POINTER(_vp), ctypes.POINTER(_vp), ctypes.c_uint32,
+                                ctypes.POINTER(_vp)],
+        "pcgpu_mlpc_release": [_vp, _vp],
+        "pcgpu_mlpc_open": [_vp, _vp, _vp, _sz, _vp, ctypes.c_uint32, _vp, _vp, _vp],
         "pcgpu_fr_from_mont": [_vp, ctypes.c_int, _vp, _vp, _sz, ctypes.c_uint32],
         "pcgpu_fr_mul": [_vp, ctypes.c_int, _vp, _vp, _vp, _sz, ctypes.c_uint32],
         "pcgpu_msm_bases": [_vp, ctypes.c_int, _vp, _vp, _vp, _sz, ctypes.c_uint32, _vp, _vp],
@@ -134,7 +149,8 @@ def _load(path):
         if fn is None:      # a library older than this binding: only the calls that need the symbol fail (AttributeError)
             continue
         fn.argtypes = args
-        fn.restype = None if name in ("pcgpu_destroy", "pcgpu_srs_release", "pcgpu_brakedown_release") else ctypes.c_int
+        fn.restype = None if name in ("pcgpu_destroy", "pcgpu_srs_release", "pcgpu_brakedown_release", "pcgpu_mlpc_release") \
+            else ctypes.c_int
     return lib
 
 
@@ -198,6 +214,24 @@ def _csc_arrays(mat):
     ind_ptr, col_ind, val = mat
     return (np.ascontiguousarray(ind_ptr, dtype=np.uint64), np.ascontiguousarray(col_ind, dtype=np.uint64),
             np.ascontiguousarray(np.asarray(val, dtype=np.uint64).reshape(-1, 4)))
+
+
+class MlpcKey:
+    """Device-resident G2 half of a MultilinearPC CommitterKey: the pair-folded powers_of_h of every level."""
+
+    def __init__(self, engine, handle, curve, nv):
+        self.engine, self.handle, self.curve, self.nv = engine, handle, curve, nv
+
+    def release(self):
+        if self.handle is not None and getattr(self.engine, "ctx", None):
+            h, self.handle = self.handle, None
+            self.engine.lib.pcgpu_mlpc_release(self.engine.ctx, h)
+
+    def __del__(self):
+        try:
+            self.release()
+        except Exception:
+            pass
 
 
 class DeviceBuffer:
@@ -328,8 +362,9 @@ class Engine:
         return g
 
     def diag_field_op(self, curve, which, op, a, b):
-        """one field primitive elementwise on the device (pcgpu_diag_field_op): which 0 = Fq, 1 = Fr of `curve`; a, b: (n, limbs)
-        uint64 Montgomery elements (limbs = 6 for BLS12-381 Fq, else 4); returns the (n, limbs) results."""
+        """one field primitive elementwise on the device (pcgpu_diag_field_op): which 0 = Fq, 1 = Fr, 2 = Fq2 of `curve`; a, b:
+        (n, limbs) uint64 Montgomery elements (limbs = 6 for BLS12-381 Fq, else 4; twice that for Fq2, c0 then c1); returns the
+        (n, limbs) results."""
         a, b = _u64(a), _u64(b)
         if a.shape != b.shape:
             raise ValueError("operand shapes differ")
@@ -341,7 +376,7 @@ class Engine:
     def srs_register(self, curve, bases_xy, inf=None, n=None, flags=0):
         bases_xy = _u64(bases_xy)
         if n is None:
-            n = bases_xy.size // (2 * fq_limbs(curve))
+            n = bases_xy.size // affine_limbs(curve)
         inf = None if inf is None else np.ascontiguousarray(inf, dtype=np.uint8)
         h = _vp()
         self._ck(self.lib.pcgpu_srs_register(self.ctx, curve, _ptr(bases_xy), _ptr(inf), n, flags, ctypes.byref(h)))
@@ -353,7 +388,7 @@ class Engine:
         scalars = _u64(scalars)
         if n is None:
             n = scalars.size // 4
-        out = np.zeros(2 * fq_limbs(srs.curve), dtype=np.uint64)
+        out = np.zeros(affine_limbs(srs.curve), dtype=np.uint64)
         inf = np.zeros(1, dtype=np.uint8)
         self._ck(self.lib.pcgpu_msm(self.ctx, srs.handle, base_offset, _ptr(scalars), n, flags, _ptr(out), _ptr(inf)))
         return out, int(inf[0])
@@ -391,6 +426,42 @@ class Engine:
         self._ck(self.lib.pcgpu_g1_fixed_base_mul(self.ctx, curve, _ptr(base_xy), _ptr(scalars), n, flags, _ptr(out)))
         return out
 
+    def g2_fixed_base_mul(self, group, base_xy, scalars, n=None, flags=0, out=None):
+        """h.batch_mul(scalars) in G2 (group BLS12_381_G2 / BN254_G2) -> (n, 4*limbs) uint64, identity written as zeros"""
+        base_xy, scalars = _u64(base_xy), _u64(scalars)
+        if n is None:
+            n = scalars.size // 4
+        if out is None:
+            out = np.zeros((n, affine_limbs(group)), dtype=np.uint64)
+        self._ck(self.lib.pcgpu_g2_fixed_base_mul(self.ctx, group, _ptr(base_xy), _ptr(scalars), n, flags, _ptr(out)))
+        return out
+
+    # ---- MultilinearPC ----
+    def mlpc_register(self, curve, powers_of_h, inf=None, flags=0):
+        """powers_of_h: nv arrays, level i of 2^(nv-i) G2 points ((2^(nv-i), 4*limbs) uint64, or device pointers with
+        DEVICE_PTRS); inf: None or nv flag arrays (entries may be None) -> MlpcKey"""
+        nv = len(powers_of_h)
+        levels = [_u64(h) for h in powers_of_h]
+        flags_arr = None if inf is None else [None if f is None else np.ascontiguousarray(f, dtype=np.uint8) for f in inf]
+        hp = (_vp * max(nv, 1))(*[_ptr(h) for h in levels])
+        ip = None if flags_arr is None else (_vp * max(nv, 1))(*[_ptr(f) for f in flags_arr])
+        h = _vp()
+        self._ck(self.lib.pcgpu_mlpc_register(self.ctx, curve, nv, hp, ip, flags, ctypes.byref(h)))
+        return MlpcKey(self, h, curve, nv)
+
+    def mlpc_open(self, key, evals, point, n=None, flags=0):
+        """MultilinearPC::open: evals (2^nv, 4) Montgomery Fr (or a device pointer with DEVICE_PTRS), point (nv, 4) Montgomery Fr
+        -> (proofs (nv, 4*limbs) uint64, identity flags (nv,) uint8, value (4,) uint64 Montgomery Fr = p(point))"""
+        evals, point = _u64(evals), _u64(point)
+        if n is None:
+            n = evals.size // 4
+        proofs = np.zeros((key.nv, affine_limbs(G2_OF[key.curve])), dtype=np.uint64)
+        pinf = np.zeros(key.nv, dtype=np.uint8)
+        value = np.zeros(4, dtype=np.uint64)
+        self._ck(self.lib.pcgpu_mlpc_open(self.ctx, key.handle, _ptr(evals), n, _ptr(point), flags, _ptr(proofs), _ptr(pinf),
+                                          _ptr(value)))
+        return proofs, pinf, value
+
     def g1_sample_generators(self, curve, protocol_name, n, first_index=0, flags=0, out=None):
         """InnerProductArgPC::sample_generators / HyraxPC::setup: n hash-derived points -> (n, 2*limbs) uint64"""
         name = np.frombuffer(bytes(protocol_name), dtype=np.uint8).copy()
@@ -412,10 +483,10 @@ class Engine:
         """VariableBaseMSM::msm_bigint on unregistered bases -> (xy, is_identity)"""
         bases_xy, scalars = _u64(bases_xy), _u64(scalars)
         n = scalars.size // 4
-        if bases_xy.size // (2 * fq_limbs(curve)) < n:
+        if bases_xy.size // affine_limbs(curve) < n:
             raise ValueError("fewer bases than scalars")
         inf = None if inf is None else np.ascontiguousarray(inf, dtype=np.uint8)
-        out = np.zeros(2 * fq_limbs(curve), dtype=np.uint64)
+        out = np.zeros(affine_limbs(curve), dtype=np.uint64)
         oinf = np.zeros(1, dtype=np.uint8)
         self._ck(self.lib.pcgpu_msm_bases(self.ctx, curve, _ptr(bases_xy), _ptr(inf), _ptr(scalars), n, flags, _ptr(out), _ptr(oinf)))
         return out, bool(oinf[0])

@@ -50,6 +50,8 @@ static void release_after_stream(pcgpu_ctx *ctx, F free_buffers) {
 PCGPU_INSTANTIATE(Bls12381, extern)
 PCGPU_INSTANTIATE(Bn254, extern)
 PCGPU_INSTANTIATE(Pallas, extern)
+PCGPU_INSTANTIATE_G2(Bls12381G2, extern)
+PCGPU_INSTANTIATE_G2(Bn254G2, extern)
 
 extern "C" const char *pcgpu_strerror(int code) {
   switch (code) {
@@ -159,7 +161,7 @@ extern "C" int pcgpu_srs_register(pcgpu_ctx *ctx, int curve, const void *bases_x
     pcgpu_srs *srs = new (std::nothrow) pcgpu_srs();
     if (!srs) return PCGPU_E_OOM;
     srs->curve = curve; srs->n = n; srs->d_tables = nullptr; srs->d_folded = nullptr; srs->c = 0; srs->groups = 1; srs->d_comb = nullptr; srs->comb_c = 0;
-    int rc = [&]() -> int { DISPATCH_CURVE(curve, return srs_register_impl<C>(ctx, bases_xy, inf, n, flags, srs)); }();
+    int rc = [&]() -> int { DISPATCH_GROUP(curve, return srs_register_impl<C>(ctx, bases_xy, inf, n, flags, srs)); }();
     if (rc) { srs_free(srs); delete srs; return rc; }
     *out = srs;
     return PCGPU_OK;
@@ -178,7 +180,7 @@ extern "C" int pcgpu_srs_curve(const pcgpu_srs *srs) { return srs ? srs->curve :
 extern "C" int pcgpu_msm(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, const void *scalars, size_t n,
                          uint32_t flags, void *out_xy, uint8_t *out_inf) {
   return on_ctx(ctx, !srs || (n && !scalars) || !out_xy, [&]() -> int {
-    DISPATCH_CURVE(srs->curve, return msm_impl<C>(ctx, srs, base_offset, scalars, n, flags, out_xy, out_inf, nullptr));
+    DISPATCH_GROUP(srs->curve, return msm_impl<C>(ctx, srs, base_offset, scalars, n, flags, out_xy, out_inf, nullptr));
   });
 }
 
@@ -199,6 +201,48 @@ extern "C" int pcgpu_g1_fixed_base_mul(pcgpu_ctx *ctx, int curve, const void *ba
                                        uint32_t flags, void *out_xy) {
   return on_ctx(ctx, !base_xy || (n && (!scalars || !out_xy)), [&]() -> int {
     DISPATCH_CURVE(curve, return fixed_base_impl<C>(ctx, base_xy, scalars, n, flags, out_xy));
+  });
+}
+
+extern "C" int pcgpu_g2_fixed_base_mul(pcgpu_ctx *ctx, int group, const void *base_xy, const void *scalars, size_t n,
+                                       uint32_t flags, void *out_xy) {
+  return on_ctx(ctx, !base_xy || (n && (!scalars || !out_xy)), [&]() -> int {
+    switch (group) {
+      case PCGPU_BLS12_381_G2: return fixed_base_impl<Bls12381G2>(ctx, base_xy, scalars, n, flags, out_xy);
+      case PCGPU_BN254_G2: return fixed_base_impl<Bn254G2>(ctx, base_xy, scalars, n, flags, out_xy);
+      default: return PCGPU_E_BADARG;
+    }
+  });
+}
+
+// ---- MultilinearPC (mlpc.cuh) -------------------------------------------------------------------------------------------
+extern "C" int pcgpu_mlpc_register(pcgpu_ctx *ctx, int curve, uint32_t nv, const void *const *powers_of_h, const uint8_t *const *inf,
+                                   uint32_t flags, pcgpu_mlpc **out) {
+  const bool bad_args = !out || !powers_of_h || nv == 0 || nv > 25 || (flags & ~(uint32_t)PCGPU_DEVICE_PTRS);
+  if (ctx && out) *out = nullptr;
+  return on_ctx(ctx, bad_args, [&]() -> int {
+    pcgpu_mlpc *m = new (std::nothrow) pcgpu_mlpc();
+    if (!m) return PCGPU_E_OOM;
+    m->curve = curve; m->nv = nv;
+    m->key.curve = curve == PCGPU_BLS12_381 ? PCGPU_BLS12_381_G2 : PCGPU_BN254_G2;
+    m->key.d_tables = nullptr; m->key.d_folded = nullptr; m->key.d_comb = nullptr; m->key.comb_c = 0;
+    int rc = [&]() -> int { DISPATCH_PAIRING_G2(curve, return mlpc_register_impl<C>(ctx, nv, powers_of_h, inf, flags, m)); }();
+    if (rc) { srs_free(&m->key); delete m; return rc; }
+    *out = m;
+    return PCGPU_OK;
+  });
+}
+
+extern "C" void pcgpu_mlpc_release(pcgpu_ctx *ctx, pcgpu_mlpc *key) {
+  if (!key) return;
+  release_after_stream(ctx, [&] { srs_free(&key->key); });
+  delete key;
+}
+
+extern "C" int pcgpu_mlpc_open(pcgpu_ctx *ctx, const pcgpu_mlpc *key, const void *evals, size_t n, const void *point, uint32_t flags,
+                               void *out_proofs_xy, uint8_t *out_proofs_inf, void *out_value) {
+  return on_ctx(ctx, !key || !evals || !point || !out_proofs_xy || (flags & ~(uint32_t)PCGPU_DEVICE_PTRS), [&]() -> int {
+    DISPATCH_PAIRING_G2(key->curve, return mlpc_open_impl<C>(ctx, key, evals, n, point, flags, out_proofs_xy, out_proofs_inf, out_value));
   });
 }
 
@@ -271,7 +315,8 @@ extern "C" int pcgpu_msm_last_geometry(pcgpu_ctx *ctx, uint64_t *out, size_t len
 }
 
 extern "C" int pcgpu_diag_field_op(pcgpu_ctx *ctx, int curve, int which, int op, const void *a, const void *b, void *out, size_t n) {
-  return on_ctx(ctx, (which != 0 && which != 1) || op < 0 || op > 9 || (n && (!a || !b || !out)), [&]() -> int {
+  return on_ctx(ctx, which < 0 || which > 2 || op < 0 || op > 9 || (n && (!a || !b || !out)), [&]() -> int {
+    if (which == 2) { DISPATCH_PAIRING_G2(curve, return diag_fq2_op_impl<C>(ctx, op, a, b, out, n)); }
     DISPATCH_CURVE(curve, return diag_field_op_impl<C>(ctx, which, op, a, b, out, n));
   });
 }

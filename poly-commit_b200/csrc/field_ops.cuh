@@ -42,4 +42,33 @@ struct FieldOpBody {
   }
 };
 
+// Fq2 (which = 2): element i is 2 N words, c0 then c1.  Ops: 0 product, 2 sum, 3 difference, 4 negation, 5 inverse (through
+// the norm), 9 square; any other op gives 0 (the entry point rejects them).
+template <class P>
+PCGPU_DEV Fq2<P> field_op2(int op, const Fq2<P> &x, const Fq2<P> &y) {
+  switch (op) {
+    case 0: return fp_mul<P>(x, y);
+    case 2: return fp_add<P>(x, y);
+    case 3: return fp_sub<P>(x, y);
+    case 4: return fp_neg<P>(x);
+    case 5: return fp_inv<P>(x);
+    case 9: return fp_sqr<P>(x);
+    default: return Fq2<P>::zero();
+  }
+}
+
+template <class P>
+struct Fq2OpBody {
+  const uint32_t *a, *b; uint32_t *out; int op;
+  PCGPU_KERNEL_DEV void operator()(size_t i) const {
+    constexpr int W = Fq2<P>::WORDS;
+    Fq2<P> x, y;
+#pragma unroll
+    for (int j = 0; j < W; j++) { coord_word(x, j) = a[i * W + j]; coord_word(y, j) = b[i * W + j]; }
+    const Fq2<P> r = field_op2<P>(op, x, y);
+#pragma unroll
+    for (int j = 0; j < W; j++) out[i * W + j] = coord_word(r, j);
+  }
+};
+
 }  // namespace pcgpu

@@ -13,6 +13,7 @@
 #pragma once
 #include <stdint.h>
 #include <string.h>
+#include <type_traits>
 #include "params_gen.cuh"
 
 namespace pcgpu {
@@ -95,21 +96,51 @@ template <class P> inline HFp<P> inv(const HFp<P> &a) {  // a^(p-2)
   return acc;
 }
 
-// XYZZ point; the byte image equals the device's XYZZ<C>
+// Fq2 = Fq[u] / (u^2 + 1), c0 then c1 (the device's Fq2<P>, fq2.cuh): the coordinate field of G2.  Same function names as
+// HFp, so the point code below runs on either field.
+template <class P>
+struct HFq2 {
+  HFp<P> c0, c1;
+  static HFq2 zero() { HFq2 r; r.c0 = HFp<P>::zero(); r.c1 = r.c0; return r; }
+  static HFq2 one() { HFq2 r; r.c0 = HFp<P>::one(); r.c1 = HFp<P>::zero(); return r; }
+  bool is_zero() const { return c0.is_zero() && c1.is_zero(); }
+  bool operator==(const HFq2 &b) const { return c0 == b.c0 && c1 == b.c1; }
+};
+template <class P> inline HFq2<P> add(const HFq2<P> &a, const HFq2<P> &b) { HFq2<P> r; r.c0 = add<P>(a.c0, b.c0); r.c1 = add<P>(a.c1, b.c1); return r; }
+template <class P> inline HFq2<P> sub(const HFq2<P> &a, const HFq2<P> &b) { HFq2<P> r; r.c0 = sub<P>(a.c0, b.c0); r.c1 = sub<P>(a.c1, b.c1); return r; }
+template <class P> inline HFq2<P> mul(const HFq2<P> &a, const HFq2<P> &b) {
+  HFq2<P> r;
+  r.c0 = sub<P>(mul<P>(a.c0, b.c0), mul<P>(a.c1, b.c1));
+  r.c1 = add<P>(mul<P>(a.c0, b.c1), mul<P>(a.c1, b.c0));
+  return r;
+}
+template <class P> inline HFq2<P> sqr(const HFq2<P> &a) { return mul<P>(a, a); }
+template <class P> inline HFq2<P> dbl(const HFq2<P> &a) { return add<P>(a, a); }
+template <class P> inline HFq2<P> inv(const HFq2<P> &a) {   // conjugate over the norm; 0 -> 0
+  const HFp<P> t = inv<P>(add<P>(mul<P>(a.c0, a.c0), mul<P>(a.c1, a.c1)));
+  HFq2<P> r;
+  r.c0 = mul<P>(a.c0, t);
+  r.c1 = sub<P>(HFp<P>::zero(), mul<P>(a.c1, t));
+  return r;
+}
+
+// XYZZ point; the byte image equals the device's XYZZ<C>.  F: HFp<Fq> for G1, HFq2<Fq> for G2 (C::EXT)
 template <class C>
 struct HXYZZ {
   using Q = typename C::Fq;
-  HFp<Q> x, y, zz, zzz;
+  using F = typename std::conditional<C::EXT == 2, HFq2<Q>, HFp<Q>>::type;
+  F x, y, zz, zzz;
   bool is_inf() const { return zz.is_zero(); }
   static HXYZZ inf() { HXYZZ p; memset(&p, 0, sizeof p); return p; }
 };
 
 template <class C> inline HXYZZ<C> pdbl(const HXYZZ<C> &p) {  // dbl-2008-s-1
   using Q = typename C::Fq;
+  using F = typename HXYZZ<C>::F;
   if (p.is_inf()) return p;
   HXYZZ<C> r;
-  HFp<Q> U = dbl<Q>(p.y), V = sqr<Q>(U), W = mul<Q>(U, V), S = mul<Q>(p.x, V);
-  HFp<Q> X2 = sqr<Q>(p.x), M = add<Q>(dbl<Q>(X2), X2);
+  F U = dbl<Q>(p.y), V = sqr<Q>(U), W = mul<Q>(U, V), S = mul<Q>(p.x, V);
+  F X2 = sqr<Q>(p.x), M = add<Q>(dbl<Q>(X2), X2);
   r.x = sub<Q>(sqr<Q>(M), dbl<Q>(S));
   r.y = sub<Q>(mul<Q>(M, sub<Q>(S, r.x)), mul<Q>(W, p.y));
   r.zz = mul<Q>(V, p.zz); r.zzz = mul<Q>(W, p.zzz);
@@ -117,12 +148,13 @@ template <class C> inline HXYZZ<C> pdbl(const HXYZZ<C> &p) {  // dbl-2008-s-1
 }
 template <class C> inline HXYZZ<C> padd(const HXYZZ<C> &p, const HXYZZ<C> &q) {  // add-2008-s
   using Q = typename C::Fq;
+  using F = typename HXYZZ<C>::F;
   if (q.is_inf()) return p;
   if (p.is_inf()) return q;
-  HFp<Q> U1 = mul<Q>(p.x, q.zz), U2 = mul<Q>(q.x, p.zz), S1 = mul<Q>(p.y, q.zzz), S2 = mul<Q>(q.y, p.zzz);
-  HFp<Q> Pd = sub<Q>(U2, U1), R = sub<Q>(S2, S1);
+  F U1 = mul<Q>(p.x, q.zz), U2 = mul<Q>(q.x, p.zz), S1 = mul<Q>(p.y, q.zzz), S2 = mul<Q>(q.y, p.zzz);
+  F Pd = sub<Q>(U2, U1), R = sub<Q>(S2, S1);
   if (Pd.is_zero()) return R.is_zero() ? pdbl<C>(p) : HXYZZ<C>::inf();
-  HFp<Q> PP = sqr<Q>(Pd), PPP = mul<Q>(Pd, PP), Qv = mul<Q>(U1, PP);
+  F PP = sqr<Q>(Pd), PPP = mul<Q>(Pd, PP), Qv = mul<Q>(U1, PP);
   HXYZZ<C> r;
   r.x = sub<Q>(sub<Q>(sqr<Q>(R), PPP), dbl<Q>(Qv));
   r.y = sub<Q>(mul<Q>(R, sub<Q>(Qv, r.x)), mul<Q>(S1, PPP));
@@ -133,21 +165,22 @@ template <class C> inline HXYZZ<C> padd(const HXYZZ<C> &p, const HXYZZ<C> &q) { 
 // affine x||y (zeros + flag for the identity)
 template <class C> inline void to_affine(const HXYZZ<C> &p, void *out_xy, uint8_t *out_inf) {
   using Q = typename C::Fq;
-  constexpr size_t FB = sizeof(HFp<Q>);
+  using F = typename HXYZZ<C>::F;
+  constexpr size_t FB = sizeof(F);
   if (p.is_inf()) { if (out_xy) memset(out_xy, 0, 2 * FB); if (out_inf) *out_inf = 1; return; }
-  HFp<Q> iv = inv<Q>(mul<Q>(p.zz, p.zzz));
-  HFp<Q> x = mul<Q>(p.x, mul<Q>(iv, p.zzz)), y = mul<Q>(p.y, mul<Q>(iv, p.zz));
-  if (out_xy) { memcpy(out_xy, x.l, FB); memcpy((char *)out_xy + FB, y.l, FB); }
+  F iv = inv<Q>(mul<Q>(p.zz, p.zzz));
+  F x = mul<Q>(p.x, mul<Q>(iv, p.zzz)), y = mul<Q>(p.y, mul<Q>(iv, p.zz));
+  if (out_xy) { memcpy(out_xy, &x, FB); memcpy((char *)out_xy + FB, &y, FB); }
   if (out_inf) *out_inf = 0;
 }
 
 // k * P for an affine P (x||y Montgomery limbs, identity = all zero) and a CANONICAL 256-bit scalar
 template <class C> inline HXYZZ<C> pmul_affine(const void *p_xy, const uint64_t *k) {
-  using Q = typename C::Fq;
+  using F = typename HXYZZ<C>::F;
   HXYZZ<C> base;
   memcpy(&base.x, p_xy, sizeof base.x); memcpy(&base.y, (const char *)p_xy + sizeof base.x, sizeof base.y);
   if (base.x.is_zero() && base.y.is_zero()) return HXYZZ<C>::inf();
-  base.zz = HFp<Q>::one(); base.zzz = HFp<Q>::one();
+  base.zz = F::one(); base.zzz = F::one();
   HXYZZ<C> acc = HXYZZ<C>::inf();
   for (int b = 255; b >= 0; b--) { acc = pdbl<C>(acc); if ((k[b >> 6] >> (b & 63)) & 1) acc = padd<C>(acc, base); }
   return acc;

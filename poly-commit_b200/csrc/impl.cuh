@@ -27,13 +27,14 @@
 #include "hash.cuh"
 #include "sprs.cuh"
 #include "field_ops.cuh"
+#include "mlpc.cuh"
 
 using namespace pcgpu;
 
 // ---------------------------------------------------------------------------------------------
 // profiling (CUDA events on the launching stream)
 // ---------------------------------------------------------------------------------------------
-enum { PROF_STAGES = 16 };
+enum { PROF_STAGES = 17 };
 struct Prof {
   bool on = false;
   double ms[PROF_STAGES] = {0};
@@ -94,7 +95,7 @@ struct pcgpu_ctx {
   uint64_t last_geom[PCGPU_GEOM_FIELDS] = {0};   // path / geometry of the most recent MSM (pcgpu_msm_last_geometry)
   std::mutex mu;
 };
-static const size_t PINNED_BYTES = 512 * 192 + 256;   // PCGPU_MAX_PLANES XYZZ<Bls12381> points + the error word
+static const size_t PINNED_BYTES = 512 * 384 + 256;   // PCGPU_MAX_PLANES XYZZ<Bls12381G2> points (the largest) + the error word
 
 static const size_t SLOT_BYTES = 256;  // >= sizeof(XYZZ<Bls12381>) = 192
 enum { PCGPU_MAX_PLANES = 512 };  // S * c of any geometry msm_geometry produces (W <= 32 windows of <= 22 bits, S <= W)
@@ -112,6 +113,25 @@ static const int NSLOTS = 8;
     case PCGPU_BN254: { using C = Bn254; CALL; }    \
     case PCGPU_PALLAS: { using C = Pallas; CALL; }  \
     default: return PCGPU_E_BADARG;                 \
+  }
+
+// the groups an MSM key can hold: the three G1s and the two G2s (include/pcgpu.h group ids)
+#define DISPATCH_GROUP(group, CALL)                          \
+  switch (group) {                                           \
+    case PCGPU_BLS12_381: { using C = Bls12381; CALL; }      \
+    case PCGPU_BN254: { using C = Bn254; CALL; }             \
+    case PCGPU_PALLAS: { using C = Pallas; CALL; }           \
+    case PCGPU_BLS12_381_G2: { using C = Bls12381G2; CALL; } \
+    case PCGPU_BN254_G2: { using C = Bn254G2; CALL; }        \
+    default: return PCGPU_E_BADARG;                          \
+  }
+
+// the G2 group of a pairing curve id (MultilinearPC, pcgpu_diag_field_op which = 2)
+#define DISPATCH_PAIRING_G2(curve, CALL)                 \
+  switch (curve) {                                       \
+    case PCGPU_BLS12_381: { using C = Bls12381G2; CALL; } \
+    case PCGPU_BN254: { using C = Bn254G2; CALL; }        \
+    default: return PCGPU_E_BADARG;                      \
   }
 
 // The operands of one call that pass through the context's staging arena.  Each operand is declared once, by what it is:
@@ -208,6 +228,7 @@ template <class C>
 int srs_register_impl(pcgpu_ctx *ctx, const void *bases, const uint8_t *inf, size_t n, uint32_t flags, pcgpu_srs *srs) {
   const size_t psz = sizeof(Affine<C>);
   uint32_t groups = 1, c = 0;
+  if (C::EXT == 2 && (flags & (PCGPU_SRS_PRECOMPUTE | PCGPU_SRS_COMB))) return PCGPU_E_BADARG;   // G2 keys hold raw bases only
   if ((flags & PCGPU_SRS_PRECOMPUTE) && n > 0) {
     c = srs_precompute_window(n);
     groups = (C::Fr::BITS + c - 1) / c;   // one table group per window (msm_geometry's W)
@@ -227,6 +248,7 @@ int srs_register_impl(pcgpu_ctx *ctx, const void *bases, const uint8_t *inf, siz
       if ((rc = io.upload())) return rc;
       if ((rc = rt::launch<256>(SrsZeroIdentityBody{(uint32_t *)srs->d_tables, d_inf, (uint32_t)(psz / 4)}, n, st))) return rc;
     }
+    if constexpr (C::EXT == 1) {
     if (groups > 1 && (rc = srs_build_groups<C>((const Affine<C> *)srs->d_tables, (uint32_t *)srs->d_folded, n, c, groups, st))) return rc;
     if (flags & PCGPU_SRS_COMB) {
       CombGeom cg; memset(&cg, 0, sizeof cg);
@@ -237,6 +259,7 @@ int srs_register_impl(pcgpu_ctx *ctx, const void *bases, const uint8_t *inf, siz
       const uint32_t chunks = (cg.NBk + COMB_CHUNK - 1) / COMB_CHUNK;
       if ((rc = rt::launch<64>(CombTableBody<C>{(const Affine<C> *)srs->d_tables, cg, (Affine<C> *)srs->d_comb, ctx->d_pow2[C::ID], chunks},
                                n * cg.W * chunks, st))) return rc;
+    }
     }
   }
   srs->c = c; srs->groups = groups;
@@ -312,7 +335,7 @@ int msm_device_planes(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, 
   rt::stream_t st = ctx->stream;
   uint32_t c, groups;
   const uint32_t *tables = (const uint32_t *)srs->d_tables;
-  uint32_t pt_words = 2 * C::Fq::N, y_words = C::Fq::N;
+  uint32_t pt_words = 2 * coord_words<typename C::F>(), y_words = coord_words<typename C::F>();
   if (srs->groups > 1 && n >= SRS_PRECOMPUTE_MIN_N) {
     c = srs->c; groups = srs->groups;
     tables = (const uint32_t *)srs->d_folded; pt_words = aligned_pt_words<C>(); y_words = aligned_y_words<C>();
@@ -325,12 +348,14 @@ int msm_device_planes(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, 
   int rc;
   // batched-affine rounds while buckets hold >= 64 points and a round still gives every thread >= 16 additions
   {
-    size_t Tmax = 0;
-    if ((rc = msm_pair_oneshot_threads<C>(&Tmax))) return rc;
-    size_t entries = (size_t)g.n * g.W, avg = entries / g.TB;
+    size_t Tmax = 0, entries = (size_t)g.n * g.W;
     uint32_t R = 0;
-    while (R < 8 && (avg >> R) >= 4 && (entries >> (R + 1)) >= 16 * Tmax) R++;
-    if (const char *e = getenv("PCGPU_MSM_AFFINE_ROUNDS")) { int v = atoi(e); if (v >= 0 && v <= 12) R = (uint32_t)v; }
+    if constexpr (C::EXT == 1) {   // G2: no batched-affine rounds (R = 0)
+      if ((rc = msm_pair_oneshot_threads<C>(&Tmax))) return rc;
+      size_t avg = entries / g.TB;
+      while (R < 8 && (avg >> R) >= 4 && (entries >> (R + 1)) >= 16 * Tmax) R++;
+      if (const char *e = getenv("PCGPU_MSM_AFFINE_ROUNDS")) { int v = atoi(e); if (v >= 0 && v <= 12) R = (uint32_t)v; }
+    }
     g.affine_rounds = R;
     uint64_t *lg = ctx->last_geom;
     memset(lg, 0, sizeof ctx->last_geom);
@@ -602,6 +627,86 @@ int fixed_base_impl(pcgpu_ctx *ctx, const void *base_xy, const void *scalars, si
   if ((rc = rt::launch<128>(FixedBaseMulBody<C>{table, d_s, d_o}, n, st))) return rc;
   if ((rc = io.download())) return rc;
   return rt::stream_sync(st);
+}
+
+// ---------------------------------------------------------------------------------------------
+// MultilinearPC (mlpc.cuh): committer key with pair-folded G2 bases, open = fold chain + nv G2 MSMs
+// ---------------------------------------------------------------------------------------------
+struct pcgpu_mlpc {
+  int curve;        // the pairing curve (PCGPU_BLS12_381 / PCGPU_BN254)
+  uint32_t nv;
+  pcgpu_srs key;    // every level's folded bases, level i at mlpc_level_offset(nv, i); key.curve is the G2 group id
+};
+
+template <class C>
+int mlpc_register_impl(pcgpu_ctx *ctx, uint32_t nv, const void *const *powers_of_h, const uint8_t *const *inf, uint32_t flags,
+                       pcgpu_mlpc *m) {
+  const size_t psz = sizeof(Affine<C>), n0 = (size_t)1 << nv;
+  rt::stream_t st = ctx->stream;
+  int rc;
+  for (uint32_t i = 0; i < nv; i++) if (!powers_of_h[i]) return PCGPU_E_BADARG;
+  if ((rc = rt::dev_malloc(&m->key.d_tables, psz * (n0 - 1)))) return rc;
+  Affine<C> *raw; uint8_t *d_inf;
+  Staging io(ctx, 0);
+  io.scratch(raw, psz * n0);
+  io.scratch(d_inf, n0);
+  if ((rc = io.upload())) return rc;
+  for (uint32_t i = 0; i < nv; i++) {
+    const size_t len = n0 >> i;
+    if (flags & PCGPU_DEVICE_PTRS) rc = rt::copy_d2d(raw, powers_of_h[i], psz * len, st);
+    else rc = rt::copy_h2d(raw, powers_of_h[i], psz * len, st);
+    if (rc) return rc;
+    if (inf && inf[i]) {
+      if (flags & PCGPU_DEVICE_PTRS) rc = rt::copy_d2d(d_inf, inf[i], len, st);
+      else rc = rt::copy_h2d(d_inf, inf[i], len, st);
+      if (rc) return rc;
+      if ((rc = rt::launch<256>(SrsZeroIdentityBody{(uint32_t *)raw, d_inf, (uint32_t)(psz / 4)}, len, st))) return rc;
+    }
+    Affine<C> *out = (Affine<C> *)m->key.d_tables + mlpc_level_offset(nv, i);
+    if ((rc = rt::launch<128>(PairFoldBasesBody<C>{raw, out}, len / 2, st))) return rc;
+    if ((rc = rt::stream_sync(st))) return rc;   // the next level's upload overwrites raw
+  }
+  m->key.n = n0 - 1; m->key.c = 0; m->key.groups = 1;
+  return PCGPU_OK;
+}
+
+template <class C>
+int mlpc_open_impl(pcgpu_ctx *ctx, const pcgpu_mlpc *m, const void *evals, size_t n, const void *point, uint32_t flags,
+                   void *out_xy, uint8_t *out_inf, void *out_value) {
+  using R = typename C::Fr;
+  const uint32_t nv = m->nv;
+  const size_t n0 = (size_t)1 << nv, psz = sizeof(Affine<C>);
+  if (n != n0) return PCGPU_E_LEN;   // "Invalid size of polynomial" (multilinear_pc/mod.rs:136)
+  rt::stream_t st = ctx->stream;
+  int rc;
+  const uint32_t *d_ev, *d_pt; uint32_t *d_q, *d_ra, *d_rb;
+  Staging io(ctx, flags);
+  io.in(d_ev, evals, n0 * 32);
+  io.host_in(d_pt, point, (size_t)nv * 32);
+  io.scratch(d_q, (n0 - 1) * 32);
+  io.scratch(d_ra, n0 / 2 * 32);
+  io.scratch(d_rb, n0 / 2 * 32);
+  if ((rc = io.upload())) return rc;
+  ctx->prof.begin(16, st);
+  const uint32_t *r = d_ev;
+  for (uint32_t i = 0; i < nv; i++) {
+    uint32_t *r_out = (i & 1) ? d_rb : d_ra;
+    if ((rc = rt::launch<256>(MlpcFoldBody<R>{r, d_pt, i, d_q + mlpc_level_offset(nv, i) * 8, r_out}, n0 >> (i + 1), st))) return rc;
+    r = r_out;
+  }
+  ctx->prof.end(16, st);
+  uint32_t value[8];
+  if ((rc = rt::copy_d2h(value, r, 32, st))) return rc;
+  if ((rc = rt::stream_sync(st))) return rc;
+  ctx->prof.collect();
+  if (out_value) memcpy(out_value, value, 32);
+  for (uint32_t i = 0; i < nv; i++) {   // the levels are independent now: level i is sum_b q_i[b] H'_i[b]
+    const size_t off = mlpc_level_offset(nv, i);
+    host::HXYZZ<C> res;
+    if ((rc = msm_to_host<C>(ctx, &m->key, off, d_q + off * 8, n0 >> (i + 1), true, &res))) return rc;
+    host::to_affine<C>(res, (char *)out_xy + i * psz, out_inf ? out_inf + i : nullptr);
+  }
+  return PCGPU_OK;
 }
 
 
@@ -1661,6 +1766,26 @@ static int diag_field_op_run(pcgpu_ctx *ctx, int op, const void *a, const void *
   return rt::stream_sync(st);
 }
 
+// which = 2: Fq2 of a pairing curve (C is its G2 group)
+template <class C>
+int diag_fq2_op_impl(pcgpu_ctx *ctx, int op, const void *a, const void *b, void *out, size_t n) {
+  using P = typename C::Fq;
+  if (op != 0 && op != 2 && op != 3 && op != 4 && op != 5 && op != 9) return PCGPU_E_BADARG;
+  if (n == 0) return PCGPU_OK;
+  rt::stream_t st = ctx->stream;
+  const size_t bytes = n * Fq2<P>::WORDS * 4;
+  int rc;
+  const uint32_t *da, *db; uint32_t *dout;
+  Staging io(ctx, 0);
+  io.host_in(da, a, bytes);
+  io.host_in(db, b, bytes);
+  io.out(dout, out, bytes);
+  if ((rc = io.upload())) return rc;
+  if ((rc = rt::launch<128>(Fq2OpBody<P>{da, db, dout, op}, n, st))) return rc;
+  if ((rc = io.download())) return rc;
+  return rt::stream_sync(st);
+}
+
 template <class C>
 int diag_field_op_impl(pcgpu_ctx *ctx, int which, int op, const void *a, const void *b, void *out, size_t n) {
   if (n == 0) return PCGPU_OK;
@@ -1802,6 +1927,17 @@ inline int measure_imad_peak_impl(pcgpu_ctx *ctx, double *ops_per_s) {
   EXT template int g1_serialize_impl<C>(pcgpu_ctx *, const void *, const uint8_t *, size_t, uint32_t, uint8_t *); \
   EXT template int g1_deserialize_impl<C>(pcgpu_ctx *, const uint8_t *, size_t, uint32_t, void *, uint8_t *, size_t *, int *); \
   EXT template int g1_sample_generators_impl<C>(pcgpu_ctx *, const uint8_t *, size_t, uint64_t, size_t, uint32_t, void *);
+// G2 groups (inst_unit.cu groups 10-12, pairing curves only): the bucket pipeline's point kernels, the small MSM and the G2 entry
+// points; the pair-round kernels are never instantiated for G2
+#define PCGPU_INST_G2(C, EXT)                                                                                              \
+  EXT template int srs_register_impl<C>(pcgpu_ctx *, const void *, const uint8_t *, size_t, uint32_t, pcgpu_srs *);        \
+  EXT template int msm_impl<C>(pcgpu_ctx *, const pcgpu_srs *, size_t, const void *, size_t, uint32_t, void *, uint8_t *, void *); \
+  EXT template int fixed_base_impl<C>(pcgpu_ctx *, const void *, const void *, size_t, uint32_t, void *);                  \
+  EXT template int diag_fq2_op_impl<C>(pcgpu_ctx *, int, const void *, const void *, void *, size_t);                      \
+  EXT template int mlpc_register_impl<C>(pcgpu_ctx *, uint32_t, const void *const *, const uint8_t *const *, uint32_t, pcgpu_mlpc *); \
+  EXT template int mlpc_open_impl<C>(pcgpu_ctx *, const pcgpu_mlpc *, const void *, size_t, const void *, uint32_t, void *, uint8_t *, void *);
+#define PCGPU_INSTANTIATE_G2(C, EXT) \
+  PCGPU_INST_ACC(C, EXT) PCGPU_INST_REDUCE(C, EXT) PCGPU_INST_PIPE(C, EXT) PCGPU_INST_SMALL(C, EXT) PCGPU_INST_G2(C, EXT)
 #define PCGPU_INSTANTIATE(C, EXT) \
   PCGPU_INST_PAIR1(C, EXT) PCGPU_INST_ACC(C, EXT) PCGPU_INST_REDUCE(C, EXT) \
   PCGPU_INST_PIPE(C, EXT) PCGPU_INST_SMALL(C, EXT) PCGPU_INST_SRS(C, EXT) PCGPU_INST_FR(C, EXT) PCGPU_INST_IPA(C, EXT)

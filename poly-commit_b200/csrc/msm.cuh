@@ -278,14 +278,18 @@ struct TaskFillBody {
 // ---------------------------------------------------------------------------------------------
 template <class C>
 PCGPU_DEV Affine<C> load_affine(const Affine<C> *p) {
-  constexpr int N = C::Fq::N;
+  constexpr int N = coord_words<typename C::F>();
   const u32x4 *q = reinterpret_cast<const u32x4 *>(p);
   Affine<C> a;
   uint32_t tmp[2 * N];
 #pragma unroll
   for (int j = 0; j < 2 * N / 4; j++) { u32x4 v = q[j]; tmp[4 * j] = v.x; tmp[4 * j + 1] = v.y; tmp[4 * j + 2] = v.z; tmp[4 * j + 3] = v.w; }
 #pragma unroll
-  for (int j = 0; j < N; j++) { a.x.l[j] = tmp[j]; a.y.l[j] = tmp[N + j]; }
+  for (int j = 0; j < N; j++) {
+    // G1 writes the limbs directly: routed through coord_word, ptxas schedules the IPA fold kernels differently
+    if constexpr (C::EXT == 1) { a.x.l[j] = tmp[j]; a.y.l[j] = tmp[N + j]; }
+    else { coord_word(a.x, j) = tmp[j]; coord_word(a.y, j) = tmp[N + j]; }
+  }
   return a;
 }
 
@@ -296,26 +300,26 @@ template <class C>
 PCGPU_DEV const uint32_t *table_record(const uint32_t *tables, size_t idx, const MsmGeom &g) { return tables + idx * g.pt_words; }
 template <class C>
 PCGPU_DEV Affine<C> load_table_point(const uint32_t *tables, size_t idx, const MsmGeom &g) {
-  constexpr int N = C::Fq::N;
+  constexpr int N = coord_words<typename C::F>();
   const uint32_t *rec = tables + idx * g.pt_words;
   const u32x4 *qx = reinterpret_cast<const u32x4 *>(rec), *qy = reinterpret_cast<const u32x4 *>(rec + g.y_words);
   Affine<C> a;
 #pragma unroll
   for (int j = 0; j < N / 4; j++) {
-    u32x4 v = qx[j]; a.x.l[4 * j] = v.x; a.x.l[4 * j + 1] = v.y; a.x.l[4 * j + 2] = v.z; a.x.l[4 * j + 3] = v.w;
-    u32x4 w = qy[j]; a.y.l[4 * j] = w.x; a.y.l[4 * j + 1] = w.y; a.y.l[4 * j + 2] = w.z; a.y.l[4 * j + 3] = w.w;
+    u32x4 v = qx[j]; coord_word(a.x, 4 * j) = v.x; coord_word(a.x, 4 * j + 1) = v.y; coord_word(a.x, 4 * j + 2) = v.z; coord_word(a.x, 4 * j + 3) = v.w;
+    u32x4 w = qy[j]; coord_word(a.y, 4 * j) = w.x; coord_word(a.y, 4 * j + 1) = w.y; coord_word(a.y, 4 * j + 2) = w.z; coord_word(a.y, 4 * j + 3) = w.w;
   }
   return a;
 }
 template <class C>
 PCGPU_DEV void store_table_point(uint32_t *tables, size_t idx, uint32_t pt_words, uint32_t y_words, const Affine<C> &a) {
-  constexpr int N = C::Fq::N;
+  constexpr int N = coord_words<typename C::F>();
   uint32_t *rec = tables + idx * pt_words;
   u32x4 *qx = reinterpret_cast<u32x4 *>(rec), *qy = reinterpret_cast<u32x4 *>(rec + y_words);
 #pragma unroll
   for (int j = 0; j < N / 4; j++) {
-    u32x4 v; v.x = a.x.l[4 * j]; v.y = a.x.l[4 * j + 1]; v.z = a.x.l[4 * j + 2]; v.w = a.x.l[4 * j + 3]; qx[j] = v;
-    u32x4 w; w.x = a.y.l[4 * j]; w.y = a.y.l[4 * j + 1]; w.z = a.y.l[4 * j + 2]; w.w = a.y.l[4 * j + 3]; qy[j] = w;
+    u32x4 v; v.x = coord_word(a.x, 4 * j); v.y = coord_word(a.x, 4 * j + 1); v.z = coord_word(a.x, 4 * j + 2); v.w = coord_word(a.x, 4 * j + 3); qx[j] = v;
+    u32x4 w; w.x = coord_word(a.y, 4 * j); w.y = coord_word(a.y, 4 * j + 1); w.z = coord_word(a.y, 4 * j + 2); w.w = coord_word(a.y, 4 * j + 3); qy[j] = w;
   }
 }
 template <class C> constexpr uint32_t aligned_pt_words() { return C::Fq::N == 12 ? 32u : 2u * C::Fq::N; }
@@ -323,7 +327,7 @@ template <class C> constexpr uint32_t aligned_y_words() { return C::Fq::N == 12 
 
 template <class C>
 PCGPU_DEV void store_xyzz(XYZZ<C> *dst, const XYZZ<C> &p) {
-  constexpr int N = C::Fq::N;
+  constexpr int N = coord_words<typename C::F>();
   u32x4 *q = reinterpret_cast<u32x4 *>(dst);
   const uint32_t *src = reinterpret_cast<const uint32_t *>(&p);
 #pragma unroll
@@ -332,7 +336,7 @@ PCGPU_DEV void store_xyzz(XYZZ<C> *dst, const XYZZ<C> &p) {
 
 template <class C>
 PCGPU_DEV XYZZ<C> load_xyzz(const XYZZ<C> *src) {
-  constexpr int N = C::Fq::N;
+  constexpr int N = coord_words<typename C::F>();
   const u32x4 *q = reinterpret_cast<const u32x4 *>(src);
   XYZZ<C> p;
   uint32_t *dst = reinterpret_cast<uint32_t *>(&p);
@@ -674,7 +678,7 @@ inline int msm_run(const uint32_t *tables, const MsmGeom &g, const uint32_t *d_s
 
   // ---- batched-affine pairwise rounds (msm_affine.cuh): halve every bucket g.affine_rounds times ----
   const Affine<C> *pts = nullptr;
-  if (g.affine_rounds && pow2) {
+  if constexpr (C::EXT == 1) if (g.affine_rounds && pow2) {   // G2 (C::EXT == 2) runs with R = 0: no pair-round kernels
     using QF = Fp<typename C::Fq>;
     size_t bound0 = max_entries / 2 + g.TB + 1, bound1 = bound0 / 2 + g.TB + 1;
     uint32_t *offA = arena.take<uint32_t>(g.TB + 2), *offB = arena.take<uint32_t>(g.TB + 2), *cnt = arena.take<uint32_t>(g.TB + 2);
