@@ -96,9 +96,9 @@ extern "C" int pcgpu_init(int device, pcgpu_ctx **out) {
   ctx->own_stream = nullptr;
 #endif
   ctx->stream = ctx->own_stream;
-  int rc = rt::dev_malloc(&ctx->d_slots, SLOT_BYTES * (NSLOTS + 2));
+  int rc = rt::dev_malloc((void **)&ctx->d_words, sizeof(DeviceWords));
   if (rc) { delete ctx; return rc; }
-  if ((rc = rt::host_alloc_pinned(&ctx->h_pinned, PINNED_BYTES))) { rt::dev_free(ctx->d_slots); delete ctx; return rc; }
+  if ((rc = rt::host_alloc_pinned((void **)&ctx->h_pinned, sizeof(PinnedZone)))) { rt::dev_free(ctx->d_words); delete ctx; return rc; }
   *out = ctx;
   return PCGPU_OK;
   });
@@ -117,7 +117,7 @@ extern "C" void pcgpu_destroy(pcgpu_ctx *ctx) {
   ctx->msm_arena.release();
   ctx->stage.release();
   ctx->ipa_arena.release();
-  rt::dev_free(ctx->d_slots);
+  rt::dev_free(ctx->d_words);
   rt::host_free_pinned(ctx->h_pinned);
   if (ctx->ev_ok) rt::event_destroy(ctx->ev_upload);
 #ifndef PCGPU_EMUL
@@ -577,7 +577,7 @@ extern "C" int pcgpu_peer_signal(pcgpu_ctx *ctx, void *const *win, uint32_t rank
 extern "C" int pcgpu_peer_wait(pcgpu_ctx *ctx, void *local_win, uint32_t world, uint32_t channel, uint64_t epoch) {
   return on_ctx(ctx, !local_win || world == 0 || world > (uint32_t)PEER_MAX_WORLD || channel >= 8, [&]() -> int {
     rt::stream_t st = ctx->stream;
-    uint32_t *d_timeout = (uint32_t *)((char *)ctx->d_slots + SLOT_BYTES * NSLOTS);
+    uint32_t *d_timeout = &ctx->d_words->peer_timeout;
     int rc;
     if ((rc = rt::dev_memset(d_timeout, 0, 4, st))) return rc;
     if ((rc = rt::launch<32>(PeerWaitBody{(const char *)local_win, world, (uint32_t)PEER_FLAG_OFFSET + 256u * channel, epoch, PEER_WAIT_CYCLES, d_timeout}, world, st))) return rc;

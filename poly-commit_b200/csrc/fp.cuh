@@ -607,6 +607,7 @@ struct Pow2TableBody {
     }
   }
 };
+template <class P> constexpr size_t pow2_table_bytes() { return (size_t)(64 * P::N + 1) * P::N * 4; }
 
 // multiply by a small constant (2, 3, 4, 8) through additions
 template <class P> PCGPU_DEV Fp<P> fp_mul3(const Fp<P> &a) { return fp_add<P>(fp_dbl<P>(a), a); }

@@ -77,6 +77,22 @@ struct pcgpu_srs {
   uint32_t comb_c;   // comb window bits
 };
 
+enum { PCGPU_MAX_PLANES = 512 };  // S * c of any geometry msm_geometry produces (W <= 32 windows of <= 22 bits, S <= W)
+
+// Page-locked landing zone of msm_issue's asynchronous copies: the S*c plane sums, packed, then msm_run's error words.
+struct PinnedZone {
+  unsigned char planes[PCGPU_MAX_PLANES * sizeof(XYZZ<Bls12381G2>)];   // sized for the largest XYZZ
+  uint32_t err[MSM_ERR_WORDS];
+};
+
+// A context's own device words.
+struct DeviceWords {
+  XYZZ<Bls12381> peer_partial;       // msm_peer_impl: a partial finished on the host, pushed as a one-plane record (largest G1)
+  uint32_t peer_timeout;             // PeerWaitBody: non-zero when a peer missed the deadline
+  unsigned long long last_nonzero;   // FrLastNonzeroBody: one past the last non-zero coefficient
+  uint32_t selftest_bad;             // FieldSelfTestBody: mismatch count
+};
+
 struct pcgpu_ctx {
   int device;
   rt::stream_t own_stream, stream;
@@ -84,22 +100,17 @@ struct pcgpu_ctx {
   rt::Arena ipa_arena;             // state of the (one) InnerProductArgPC::open in progress on this context; reused across opens
   bool ipa_active = false;
   uint32_t pair_tdiv = 1;          // set by the batch entry points while several pipelines are in flight (msm_run)
-  void *d_slots;    // 8 XYZZ result slots + 1 affine + err word, generously sized
+  DeviceWords *d_words = nullptr;
   Prof prof;
   uint32_t *d_pow2[3] = {nullptr, nullptr, nullptr};  // fp_inv_gcd tables (Fq), per curve
   std::vector<pcgpu_ctx *> siblings;  // extra contexts on the same device for pcgpu_kzg_commit_batch
   std::vector<NttPlan> ntt_plans;  // twiddle tables, cached per (curve, logn, direction)
-  void *h_pinned = nullptr;        // page-locked landing zone of the asynchronous plane / error-word copies (PINNED_BYTES)
+  PinnedZone *h_pinned = nullptr;
   rt::event_t ev_upload;           // "inputs are on the device": lets a sibling context's stream start on them
   bool ev_ok = false;
   uint64_t last_geom[PCGPU_GEOM_FIELDS] = {0};   // path / geometry of the most recent MSM (pcgpu_msm_last_geometry)
   std::mutex mu;
 };
-static const size_t PINNED_BYTES = 512 * 384 + 256;   // PCGPU_MAX_PLANES XYZZ<Bls12381G2> points (the largest) + the error word
-
-static const size_t SLOT_BYTES = 256;  // >= sizeof(XYZZ<Bls12381>) = 192
-enum { PCGPU_MAX_PLANES = 512 };  // S * c of any geometry msm_geometry produces (W <= 32 windows of <= 22 bits, S <= W)
-static const int NSLOTS = 8;
 
 #ifndef PCGPU_EMUL
 #define SET_DEVICE(ctx) do { if (cudaSetDevice((ctx)->device) != cudaSuccess) return PCGPU_E_CUDA; } while (0)
@@ -158,7 +169,7 @@ class Staging {
 
  private:
   enum { TO_DEV = 1, TO_HOST = 2, MAX_OPS = 8 };
-  struct Op { void *slot; void (*set)(void *slot, void *p); const void *src; void *dst; size_t bytes; int copy; void *buf; };
+  struct Op { void *slot; void (*set)(void *slot, void *p); const void *src; void *dst; size_t bytes; int copy; char *buf; };
   template <class P> void add(P &d, bool callers, const void *src, void *dst, size_t bytes, int copy) {
     if (callers) { d = static_cast<P>(const_cast<void *>(src)); return; }
     if (n_ == MAX_OPS) { overflow_ = true; return; }
@@ -172,17 +183,11 @@ class Staging {
 
 inline int Staging::upload() {
   if (overflow_) return PCGPU_E_BADARG;
-  size_t need = 0;
-  for (int i = 0; i < n_; i++) need += rt::Arena::pad(ops_[i].bytes ? ops_[i].bytes : 1);
-  int rc = ctx_->stage.reserve(need);
+  int rc = ctx_->stage.carve([&](auto &&buf) { for (int i = 0; i < n_; i++) buf(ops_[i].buf, ops_[i].bytes); });
   if (rc) return rc;
   for (int i = 0; i < n_; i++) {
-    Op &o = ops_[i];
-    if (!(o.buf = ctx_->stage.take<char>(o.bytes ? o.bytes : 1))) return PCGPU_E_OOM;
-    o.set(o.slot, o.buf);
-  }
-  for (int i = 0; i < n_; i++) {
     const Op &o = ops_[i];
+    o.set(o.slot, o.buf);
     if ((o.copy & TO_DEV) && o.bytes && (rc = rt::copy_h2d(o.buf, o.src, o.bytes, ctx_->stream))) return rc;
   }
   return PCGPU_OK;
@@ -294,10 +299,9 @@ int msm_small_to_host(pcgpu_ctx *ctx, const MsmSmallProblem<C> *probs, uint32_t 
   memset(ctx->last_geom, 0, sizeof ctx->last_geom);
   ctx->last_geom[PCGPU_GEOM_PATH] = PCGPU_MSM_PATH_SMALL; ctx->last_geom[PCGPU_GEOM_SPLIT] = split; ctx->last_geom[PCGPU_GEOM_N] = nmax;
   const size_t npts = (size_t)nprob * W * split;
-  if ((rc = ctx->msm_arena.reserve(rt::Arena::pad(npts * sizeof(XYZZ<C>)) + 4096))) return rc;
-  uint32_t *d_err = ctx->msm_arena.take<uint32_t>(16);
-  XYZZ<C> *d_out = ctx->msm_arena.take<XYZZ<C>>(npts);
-  if ((rc = rt::dev_memset(d_err, 0, 64, st))) return rc;
+  uint32_t *d_err; XYZZ<C> *d_out;
+  if ((rc = ctx->msm_arena.carve([&](auto &&buf) { buf(d_err, 1); buf(d_out, npts); }))) return rc;
+  if ((rc = rt::dev_memset(d_err, 0, sizeof *d_err, st))) return rc;
   MsmSmallBody<C> body;
   memset(&body, 0, sizeof body);
   for (uint32_t p = 0; p < nprob; p++) body.prob[p] = probs[p];
@@ -328,7 +332,7 @@ int msm_small_to_host(pcgpu_ctx *ctx, const MsmSmallProblem<C> *probs, uint32_t 
 }
 
 // Device half of one bucket-pipeline MSM (n > SMALL_MAX_N or the small path disabled): picks the geometry, runs msm_run on
-// the context's stream and returns (asynchronously) the compact S*c bit-plane sums and the error word.
+// the context's stream and returns (asynchronously) the compact S*c bit-plane sums and the error words.
 template <class C>
 int msm_device_planes(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, const uint32_t *d_scalars, size_t n,
                              bool mont, MsmGeom *g_out, const XYZZ<C> **d_planes, size_t *stride, uint32_t **d_err) {
@@ -363,11 +367,7 @@ int msm_device_planes(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, 
     lg[PCGPU_GEOM_G] = g.G; lg[PCGPU_GEOM_R] = R; lg[PCGPU_GEOM_WAVE] = Tmax; lg[PCGPU_GEOM_ENTRIES] = entries;
     lg[PCGPU_GEOM_HEAVY] = UINT64_MAX;   // msm_collect fills it in from the pipeline's error words
   }
-  if (g.affine_rounds && !ctx->d_pow2[C::ID]) {
-    using QP = typename C::Fq;
-    if ((rc = rt::dev_malloc((void **)&ctx->d_pow2[C::ID], (size_t)(64 * QP::N + 1) * QP::N * 4))) return rc;
-    if ((rc = rt::launch<32>(Pow2TableBody<QP>{ctx->d_pow2[C::ID]}, 1, st))) return rc;
-  }
+  if (g.affine_rounds && (rc = ensure_pow2<C>(ctx))) return rc;
   *g_out = g;
   uint32_t T = 0, tdiv = 0;
   rc = msm_run<C>(tables, g, d_scalars, ctx->msm_arena, d_planes, stride, d_err, st, ctx->prof, ctx->d_pow2[C::ID], &T, &tdiv);
@@ -377,7 +377,7 @@ int msm_device_planes(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, 
 
 // One MSM in two halves so that a caller can keep several pipelines in flight from one host thread:
 //   msm_issue    launches the device pipeline on the context's stream and queues the copy of the S*c bit-plane sums (and the
-//                error word) into the context's pinned buffer -- returns without waiting
+//                error words) into the context's pinned zone -- returns without waiting
 //   msm_collect  waits for that stream and combines the planes on the host (host_ec.hpp)
 // MSMs below the small-path threshold complete inside msm_issue.
 template <class C>
@@ -403,10 +403,11 @@ int msm_issue(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, const ui
   if (rc) return rc;
   p->np = (size_t)p->g.S * p->g.c;   // one-level: c planes per set; two-level: (h+1) + (c-1-h) = c planes per set as well
   static_assert(sizeof(host::HXYZZ<C>) == sizeof(XYZZ<C>), "host/device point layouts must agree");
+  static_assert(PCGPU_MAX_PLANES * sizeof(XYZZ<C>) <= sizeof(PinnedZone::planes), "the plane sums must fit the pinned zone");
   if (p->np > PCGPU_MAX_PLANES || !ctx->h_pinned) return PCGPU_E_BADARG;
-  char *hp = (char *)ctx->h_pinned;
-  if ((rc = rt::copy_d2h_2d(hp, sizeof(XYZZ<C>), d_planes, stride * sizeof(XYZZ<C>), sizeof(XYZZ<C>), p->np, st))) return rc;
-  if ((rc = rt::copy_d2h(hp + PINNED_BYTES - 64, d_err, 16 * sizeof(uint32_t), st))) return rc;   // all of msm_run's error words
+  PinnedZone *hp = ctx->h_pinned;
+  if ((rc = rt::copy_d2h_2d(hp->planes, sizeof(XYZZ<C>), d_planes, stride * sizeof(XYZZ<C>), sizeof(XYZZ<C>), p->np, st))) return rc;
+  if ((rc = rt::copy_d2h(hp->err, d_err, sizeof hp->err, st))) return rc;
   p->done = false;
   return PCGPU_OK;
 }
@@ -417,13 +418,11 @@ int msm_collect(pcgpu_ctx *ctx, MsmPending<C> *p, host::HXYZZ<C> *out) {
   int rc = rt::stream_sync(ctx->stream);
   if (rc) return rc;
   ctx->prof.collect();
-  const char *hp = (const char *)ctx->h_pinned;
-  uint32_t herr[16];
-  memcpy(herr, hp + PINNED_BYTES - 64, sizeof herr);
-  ctx->last_geom[PCGPU_GEOM_HEAVY] = herr[12];   // err[12]: heavy buckets (msm_run)
-  if (herr[0]) return PCGPU_E_RANGE;
+  const PinnedZone *hp = ctx->h_pinned;
+  ctx->last_geom[PCGPU_GEOM_HEAVY] = hp->err[MSM_ERR_HEAVY];
+  if (hp->err[MSM_ERR_RANGE]) return PCGPU_E_RANGE;
   auto t0 = std::chrono::steady_clock::now();
-  const host::HXYZZ<C> *planes = (const host::HXYZZ<C> *)hp;
+  const host::HXYZZ<C> *planes = (const host::HXYZZ<C> *)hp->planes;
   *out = p->g.h_split ? host::combine_bit_planes_2level<C>(planes, p->g.S, p->g.c, p->g.h_split)
                       : host::combine_bit_planes<C>(planes, p->g.S, p->g.c);
   if (ctx->prof.on) {
@@ -488,7 +487,7 @@ int msm_peer_impl(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, cons
   memset(&push, 0, sizeof push);
   for (uint32_t d = 0; d < world; d++) push.win[d] = (char *)win[d];
   push.rank = rank; push.world = world; push.epoch = epoch;
-  uint32_t *d_timeout = (uint32_t *)((char *)ctx->d_slots + SLOT_BYTES * NSLOTS);
+  uint32_t *d_timeout = &ctx->d_words->peer_timeout;
   bool pipeline = n > SMALL_MAX_N || (n > 0 && !msm_small_enabled());
   MsmGeom g;
   if (pipeline) {
@@ -506,7 +505,8 @@ int msm_peer_impl(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, cons
     // small or unfolded MSM: this rank's partial is finished on the host and pushed as a one-plane record
     host::HXYZZ<C> part;
     if ((rc = msm_to_host<C>(ctx, srs, base_offset, d_scalars, n, mont, &part))) return rc;
-    XYZZ<C> *d_one = (XYZZ<C> *)ctx->d_slots;
+    static_assert(sizeof(XYZZ<C>) <= sizeof(DeviceWords::peer_partial), "the partial must fit its device slot");
+    XYZZ<C> *d_one = (XYZZ<C> *)&ctx->d_words->peer_partial;
     if ((rc = rt::copy_h2d(d_one, &part, sizeof part, st))) return rc;
     push.planes = (const uint32_t *)d_one; push.plane_words = sizeof(XYZZ<C>) / 4;
     push.hdr.np = 1; push.hdr.S = 1; push.hdr.c = 1; push.hdr.h_split = 0; push.d_err = nullptr;
@@ -938,8 +938,8 @@ static int device_trim_trailing_zeros(pcgpu_ctx *ctx, const void *d_coeffs, size
     if ((rc = rt::copy_d2h(top, (const char *)d_coeffs + (*n - 1) * 32, 32, st))) return rc;
     if ((rc = rt::stream_sync(st))) return rc;
     if (top[0] | top[1] | top[2] | top[3]) return PCGPU_OK;
-    unsigned long long *d_last = (unsigned long long *)((char *)ctx->d_slots + SLOT_BYTES * NSLOTS + 64);
-    if ((rc = rt::dev_memset(d_last, 0, 8, st))) return rc;
+    unsigned long long *d_last = &ctx->d_words->last_nonzero;
+    if ((rc = rt::dev_memset(d_last, 0, sizeof *d_last, st))) return rc;
     if ((rc = rt::launch<256>(FrLastNonzeroBody{(const uint32_t *)d_coeffs, *n, d_last}, *n, st))) return rc;
     unsigned long long h = 0;
     if ((rc = rt::copy_d2h(&h, d_last, 8, st))) return rc;
@@ -995,13 +995,19 @@ int kzg_commit_open_impl(pcgpu_ctx *ctx, pcgpu_ctx *sib, const pcgpu_srs *pg, co
 // ---------------------------------------------------------------------------------------------
 // IPA halving loop (device-resident)
 // ---------------------------------------------------------------------------------------------
+// Device buffers are carved from the context's IPA arena by ipa_begin.
 struct pcgpu_ipa {
   int curve; size_t n0, n;
-  void *d_key;        // n0 affine points (folded in place until the key is frozen)
-  uint32_t *d_coeffs, *d_z, *d_scr;  // n0 Fr each; scratch for inner products
-  pcgpu_srs view;     // non-owning SRS view over d_key for the MSM pipeline
-  size_t frozen_m;    // 0: the key is folded explicitly; else the key stays at frozen_m points (ipa.cuh, "late rounds")
-  uint32_t *d_w;      // frozen_m weights, then 2 * frozen_m MSM scalars (allocated at the freeze)
+  void *d_key;               // n0 affine points (folded in place until the key is frozen)
+  uint32_t *d_coeffs, *d_z;  // n0 Fr each
+  uint32_t *d_ip_scratch;    // fr_inner_product's scratch
+  uint32_t *d_point;         // the evaluation point z (1 Fr)
+  uint32_t *d_ip;            // <coeffs_r, z_l>, <coeffs_l, z_r> (2 Fr)
+  uint32_t *d_ch, *d_chi;    // the round's challenge and its inverse (1 Fr each)
+  void *d_h;                 // h' (one affine point)
+  pcgpu_srs view;            // non-owning SRS view over d_key for the MSM pipeline
+  size_t frozen_m;           // 0: the key is folded explicitly; else the key stays at frozen_m points (ipa.cuh, "late rounds")
+  uint32_t *d_w, *d_sl, *d_sr;   // frozen key: the weights and the l / r MSM scalars (SMALL_MAX_N Fr each)
 };
 
 template <class C>
@@ -1009,7 +1015,7 @@ static int ensure_pow2(pcgpu_ctx *ctx) {
   using QP = typename C::Fq;
   if (ctx->d_pow2[C::ID]) return PCGPU_OK;
   int rc;
-  if ((rc = rt::dev_malloc((void **)&ctx->d_pow2[C::ID], (size_t)(64 * QP::N + 1) * QP::N * 4))) return rc;
+  if ((rc = rt::dev_malloc((void **)&ctx->d_pow2[C::ID], pow2_table_bytes<QP>()))) return rc;
   return rt::launch<32>(Pow2TableBody<QP>{ctx->d_pow2[C::ID]}, 1, ctx->stream);
 }
 
@@ -1021,7 +1027,7 @@ enum { IPA_FOLD_MIN_BLOCKS = PCGPU_IPA_FOLD_MIN_BLOCKS };
 template <class C>
 static int ipa_freeze(pcgpu_ctx *ctx, pcgpu_ipa *st) {
   using R = typename C::Fr;
-  st->frozen_m = st->n;   // d_w (3 * SMALL_MAX_N elements) was carved out of the context's IPA arena by ipa_begin
+  st->frozen_m = st->n;
   return rt::launch<128>(FrFillOneBody<R>{st->d_w}, st->n, ctx->stream);
 }
 inline bool ipa_freeze_enabled() {
@@ -1036,25 +1042,24 @@ int ipa_begin_impl(pcgpu_ctx *ctx, const void *key_xy, size_t n, const void *coe
   rt::stream_t s = ctx->stream;
   int rc;
   bool dev = (flags & PCGPU_DEVICE_PTRS) != 0;
-  st->curve = C::ID; st->n0 = st->n = n;
-  st->d_key = nullptr; st->d_coeffs = nullptr; st->frozen_m = 0; st->d_w = nullptr;
+  st->curve = C::ID; st->n0 = st->n = n; st->frozen_m = 0;
   if ((rc = ensure_pow2<C>(ctx))) return rc;
   // one arena per context, grown on demand and kept: an open costs no cudaMalloc / cudaFree after the first
   if (ctx->ipa_active) return PCGPU_E_BADARG;          // one halving loop at a time per context
-  const size_t fr_words = (2 * n + IP_THREADS + IP_THREADS / IP_BLOCK + 32) * 8;
-  if ((rc = ctx->ipa_arena.reserve(rt::Arena::pad(n * sizeof(Affine<C>)) + rt::Arena::pad(fr_words * 4) + rt::Arena::pad(3 * SMALL_MAX_N * 32 + 64) + 4096))) return rc;
-  st->d_key = ctx->ipa_arena.take<Affine<C>>(n);
-  st->d_coeffs = ctx->ipa_arena.take<uint32_t>(fr_words);
-  st->d_w = ctx->ipa_arena.take<uint32_t>(3 * SMALL_MAX_N * 8 + 16);
-  if (!st->d_key || !st->d_coeffs || !st->d_w) return PCGPU_E_OOM;
+  Affine<C> *key, *h;
+  rc = ctx->ipa_arena.carve([&](auto &&buf) {
+    buf(key, n); buf(st->d_coeffs, 8 * n); buf(st->d_z, 8 * n); buf(st->d_ip_scratch, 8 * (IP_THREADS + IP_THREADS / IP_BLOCK));
+    buf(st->d_point, 8); buf(st->d_ip, 2 * 8); buf(st->d_ch, 8); buf(st->d_chi, 8); buf(h, 1);
+    buf(st->d_w, 8 * SMALL_MAX_N); buf(st->d_sl, 8 * SMALL_MAX_N); buf(st->d_sr, 8 * SMALL_MAX_N);
+  });
+  if (rc) return rc;
+  st->d_key = key; st->d_h = h;
   ctx->ipa_active = true;
-  st->d_z = st->d_coeffs + 8 * n; st->d_scr = st->d_z + 8 * n;
   if ((rc = dev ? rt::copy_d2d(st->d_key, key_xy, n * sizeof(Affine<C>), s) : rt::copy_h2d(st->d_key, key_xy, n * sizeof(Affine<C>), s))) return rc;
   if ((rc = rt::dev_memset(st->d_coeffs, 0, n * 32, s))) return rc;
   if (n_coeffs && (rc = dev ? rt::copy_d2d(st->d_coeffs, coeffs, n_coeffs * 32, s) : rt::copy_h2d(st->d_coeffs, coeffs, n_coeffs * 32, s))) return rc;
-  uint32_t *d_pt = st->d_scr + 8 * (IP_THREADS + IP_THREADS / IP_BLOCK + 4);
-  if ((rc = rt::copy_h2d(d_pt, point, 32, s))) return rc;
-  if ((rc = rt::launch<128>(FrPowersBody<R>{d_pt, st->d_z}, n, s))) return rc;
+  if ((rc = rt::copy_h2d(st->d_point, point, 32, s))) return rc;
+  if ((rc = rt::launch<128>(FrPowersBody<R>{st->d_point, st->d_z}, n, s))) return rc;
   st->view.curve = C::ID; st->view.n = n; st->view.c = 0; st->view.groups = 1; st->view.d_tables = st->d_key; st->view.d_folded = nullptr;
   st->view.d_comb = nullptr; st->view.comb_c = 0;
   if (n <= SMALL_MAX_N && n > 1 && ipa_freeze_enabled() && (rc = ipa_freeze<C>(ctx, st))) return rc;
@@ -1070,19 +1075,18 @@ int ipa_round_lr_impl(pcgpu_ctx *ctx, pcgpu_ctx *sib, pcgpu_ipa *st, const void 
   size_t m = st->n / 2;
   if (m == 0) return PCGPU_E_BADARG;
   const uint32_t *cl = st->d_coeffs, *cr = st->d_coeffs + 8 * m, *zl = st->d_z, *zr = st->d_z + 8 * m;
-  uint32_t *d_ip = st->d_scr + 8 * (IP_THREADS + IP_THREADS / IP_BLOCK + 6);
+  uint32_t *d_ip = st->d_ip, *scr = st->d_ip_scratch;
+  const Affine<C> *d_h = (const Affine<C> *)st->d_h;
   uint64_t ip_m[2][4], ip_c[2][4];
   if (st->frozen_m) {
     // frozen key: both commitments are frozen_m-term MSMs over the same points, scalars expanded on the device
     const size_t M = st->frozen_m;
-    uint32_t *d_h = st->d_scr + 8 * (IP_THREADS + IP_THREADS / IP_BLOCK + 12);
-    uint32_t *s_l = st->d_w + 8 * M, *s_r = s_l + 8 * M;
-    if ((rc = fr_inner_product<R>(cr, zl, m, d_ip, st->d_scr, s))) return rc;
-    if ((rc = fr_inner_product<R>(cl, zr, m, d_ip + 8, st->d_scr, s))) return rc;
-    if ((rc = rt::copy_h2d(d_h, h_prime_xy, sizeof(Affine<C>), s))) return rc;
-    if ((rc = rt::launch<128>(IpaFrozenScalarsBody<R>{st->d_w, st->d_coeffs, (uint32_t)st->n, s_l, s_r}, M, s))) return rc;
+    if ((rc = fr_inner_product<R>(cr, zl, m, d_ip, scr, s))) return rc;
+    if ((rc = fr_inner_product<R>(cl, zr, m, d_ip + 8, scr, s))) return rc;
+    if ((rc = rt::copy_h2d(st->d_h, h_prime_xy, sizeof(Affine<C>), s))) return rc;
+    if ((rc = rt::launch<128>(IpaFrozenScalarsBody<R>{st->d_w, st->d_coeffs, (uint32_t)st->n, st->d_sl, st->d_sr}, M, s))) return rc;
     const Affine<C> *key = (const Affine<C> *)st->d_key;
-    MsmSmallProblem<C> pr[2] = {{key, s_l, (const Affine<C> *)d_h, d_ip, (uint32_t)M}, {key, s_r, (const Affine<C> *)d_h, d_ip + 8, (uint32_t)M}};
+    MsmSmallProblem<C> pr[2] = {{key, st->d_sl, d_h, d_ip, (uint32_t)M}, {key, st->d_sr, d_h, d_ip + 8, (uint32_t)M}};
     host::HXYZZ<C> lr[2];
     if ((rc = msm_small_to_host<C>(ctx, pr, 2, true, lr))) return rc;
     host::to_affine<C>(lr[0], out_l_xy, out_l_inf);
@@ -1091,13 +1095,12 @@ int ipa_round_lr_impl(pcgpu_ctx *ctx, pcgpu_ctx *sib, pcgpu_ipa *st, const void 
   }
   if (m <= 2 * SMALL_MAX_N && msm_small_enabled()) {
     // rounds of <= 8192-term commitments (the bucket pipeline's fixed cost dominates at this size): both commitments, each with its  + h' * <.,.>  term, in ONE launch; the inner products never leave HBM
-    uint32_t *d_h = st->d_scr + 8 * (IP_THREADS + IP_THREADS / IP_BLOCK + 12);   // 3 slots, clear of d_ip / d_ch
-    if ((rc = fr_inner_product<R>(cr, zl, m, d_ip, st->d_scr, s))) return rc;
-    if ((rc = fr_inner_product<R>(cl, zr, m, d_ip + 8, st->d_scr, s))) return rc;
-    if ((rc = rt::copy_h2d(d_h, h_prime_xy, sizeof(Affine<C>), s))) return rc;
+    if ((rc = fr_inner_product<R>(cr, zl, m, d_ip, scr, s))) return rc;
+    if ((rc = fr_inner_product<R>(cl, zr, m, d_ip + 8, scr, s))) return rc;
+    if ((rc = rt::copy_h2d(st->d_h, h_prime_xy, sizeof(Affine<C>), s))) return rc;
     const Affine<C> *key = (const Affine<C> *)st->view.d_tables;
-    MsmSmallProblem<C> pr[2] = {{key, cr, (const Affine<C> *)d_h, d_ip, (uint32_t)m},          // cm_commit(key_l, coeffs_r) + h' <c_r, z_l>
-                                {key + m, cl, (const Affine<C> *)d_h, d_ip + 8, (uint32_t)m}};  // cm_commit(key_r, coeffs_l) + h' <c_l, z_r>
+    MsmSmallProblem<C> pr[2] = {{key, cr, d_h, d_ip, (uint32_t)m},          // cm_commit(key_l, coeffs_r) + h' <c_r, z_l>
+                                {key + m, cl, d_h, d_ip + 8, (uint32_t)m}};  // cm_commit(key_r, coeffs_l) + h' <c_l, z_r>
     host::HXYZZ<C> lr[2];
     if ((rc = msm_small_to_host<C>(ctx, pr, 2, true, lr))) return rc;
     host::to_affine<C>(lr[0], out_l_xy, out_l_inf);
@@ -1106,8 +1109,8 @@ int ipa_round_lr_impl(pcgpu_ctx *ctx, pcgpu_ctx *sib, pcgpu_ipa *st, const void 
   }
   // <coeffs_r, z_l>, <coeffs_l, z_r> (results fetched after the MSMs have been queued), then the two commitments: cm_commit(key_l,
   // coeffs_r) on this context's stream and cm_commit(key_r, coeffs_l) on the sibling's, so their latency-bound stages overlap
-  if ((rc = fr_inner_product<R>(cr, zl, m, d_ip, st->d_scr, s))) return rc;
-  if ((rc = fr_inner_product<R>(cl, zr, m, d_ip + 8, st->d_scr, s))) return rc;   // stream order: the first product is complete
+  if ((rc = fr_inner_product<R>(cr, zl, m, d_ip, scr, s))) return rc;
+  if ((rc = fr_inner_product<R>(cl, zr, m, d_ip + 8, scr, s))) return rc;   // stream order: the first product is complete
   if ((rc = rt::copy_d2h(ip_m[0], d_ip, 32, s))) return rc;
   if ((rc = rt::copy_d2h(ip_m[1], d_ip + 8, 32, s))) return rc;
   host::HXYZZ<C> l, r;
@@ -1138,13 +1141,12 @@ int ipa_round_fold_impl(pcgpu_ctx *ctx, pcgpu_ipa *st, const void *challenge, co
   int rc;
   size_t m = st->n / 2;
   if (m == 0) return PCGPU_E_BADARG;
-  uint32_t *d_ch = st->d_scr + 8 * (IP_THREADS + IP_THREADS / IP_BLOCK + 8), *d_chi = d_ch + 8;
-  if ((rc = rt::copy_h2d(d_ch, challenge, 32, s))) return rc;
-  if ((rc = rt::copy_h2d(d_chi, challenge_inv, 32, s))) return rc;
-  if ((rc = rt::launch<256>(FrAxpyBody<R>{st->d_coeffs, d_chi, st->d_coeffs + 8 * m}, m, s))) return rc;  // :691-693
-  if ((rc = rt::launch<256>(FrAxpyBody<R>{st->d_z, d_ch, st->d_z + 8 * m}, m, s))) return rc;              // :695-697
+  if ((rc = rt::copy_h2d(st->d_ch, challenge, 32, s))) return rc;
+  if ((rc = rt::copy_h2d(st->d_chi, challenge_inv, 32, s))) return rc;
+  if ((rc = rt::launch<256>(FrAxpyBody<R>{st->d_coeffs, st->d_chi, st->d_coeffs + 8 * m}, m, s))) return rc;  // :691-693
+  if ((rc = rt::launch<256>(FrAxpyBody<R>{st->d_z, st->d_ch, st->d_z + 8 * m}, m, s))) return rc;              // :695-697
   if (st->frozen_m) {   // the key's fold is a multiplication of the weights (ipa.cuh)
-    if ((rc = rt::launch<128>(IpaFrozenWeightBody<R>{st->d_w, d_ch, (uint32_t)st->n}, st->frozen_m, s))) return rc;
+    if ((rc = rt::launch<128>(IpaFrozenWeightBody<R>{st->d_w, st->d_ch, (uint32_t)st->n}, st->frozen_m, s))) return rc;
     st->n = m;
     return rt::stream_sync(s);
   }
@@ -1741,7 +1743,7 @@ struct FieldSelfTestBody {
 template <class C, class P>
 static int diag_field_op_run(pcgpu_ctx *ctx, int op, const void *a, const void *b, void *out, size_t n) {
   rt::stream_t st = ctx->stream;
-  const size_t bytes = n * P::N * 4, tbytes = (size_t)(64 * P::N + 1) * P::N * 4;
+  const size_t bytes = n * P::N * 4;
   int rc;
   const bool fr_table = op == 8 && !std::is_same<P, typename C::Fq>::value;   // no kernel inverts in Fr by binary GCD
   const uint32_t *da, *db; uint32_t *dout, *t = nullptr;
@@ -1749,7 +1751,7 @@ static int diag_field_op_run(pcgpu_ctx *ctx, int op, const void *a, const void *
   io.host_in(da, a, bytes);
   io.host_in(db, b, bytes);
   io.out(dout, out, bytes);
-  if (fr_table) io.scratch(t, tbytes);   // a table for this call only
+  if (fr_table) io.scratch(t, pow2_table_bytes<P>());   // a table for this call only
   if ((rc = io.upload())) return rc;
   const uint32_t *pow2 = nullptr;
   if (op == 8) {
@@ -1797,8 +1799,8 @@ template <class C>
 int selftest_field_impl(pcgpu_ctx *ctx, uint64_t seed, size_t n, uint64_t *mismatches) {
   rt::stream_t st = ctx->stream;
   int rc;
-  uint32_t *d_bad = (uint32_t *)((char *)ctx->d_slots + SLOT_BYTES * (NSLOTS + 1));
-  if ((rc = rt::dev_memset(d_bad, 0, 8, st))) return rc;
+  uint32_t *d_bad = &ctx->d_words->selftest_bad;
+  if ((rc = rt::dev_memset(d_bad, 0, sizeof *d_bad, st))) return rc;
   if ((rc = rt::launch<128>(FieldSelfTestBody<typename C::Fq>{seed, d_bad}, n, st))) return rc;
   if ((rc = rt::launch<128>(FieldSelfTestBody<typename C::Fr>{seed ^ 0x5555, d_bad}, n, st))) return rc;
   uint32_t h = 0;

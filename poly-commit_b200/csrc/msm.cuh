@@ -571,28 +571,13 @@ inline size_t msm_plane_scratch_elems(const MsmGeom &g) {
   return (size_t)g.S * (rows + cols);
 }
 
-template <class C>
-inline size_t msm_workspace_bytes(const MsmGeom &g) {
-  size_t max_entries = (size_t)g.n * g.W;
-  size_t max_tasks = max_entries / g.L + g.TB + 1;
-  size_t b = 0;
-  b += 5 * rt::Arena::pad((g.TB + 2) * sizeof(uint32_t));
-  b += rt::Arena::pad(max_tasks * sizeof(uint32_t));
-  b += rt::Arena::pad((max_entries + 1) * sizeof(uint32_t));
-  b += rt::Arena::pad(scan_scratch_words(g.TB + 1) * sizeof(uint32_t));
-  b += rt::Arena::pad(64);
-  b += rt::Arena::pad(max_tasks * sizeof(XYZZ<C>));
-  b += rt::Arena::pad((size_t)g.TB * sizeof(XYZZ<C>));
-  b += rt::Arena::pad(msm_plane_scratch_elems(g) * sizeof(XYZZ<C>)) + rt::Arena::pad((size_t)g.S * 2 * g.c * sizeof(XYZZ<C>));
-  if (g.affine_rounds) {
-    size_t bound0 = max_entries / 2 + g.TB + 1, bound1 = bound0 / 2 + g.TB + 1;
-    b += 3 * rt::Arena::pad((g.TB + 2) * sizeof(uint32_t));
-    b += rt::Arena::pad(bound0 * sizeof(uint32_t));
-    b += rt::Arena::pad(3 * (bound0 + (1u << 20)) * sizeof(Fp<typename C::Fq>));
-    b += rt::Arena::pad(bound0 * sizeof(Affine<C>)) + rt::Arena::pad(bound1 * sizeof(Affine<C>));
-  }
-  return b + 4096;
-}
+// msm_run's error words: MSM_ERR_WORDS uint32 on the device, zeroed by every run
+enum {
+  MSM_ERR_RANGE = 0,    // non-zero: a scalar was out of range
+  MSM_ERR_QUEUE = 8,    // the accumulate kernel's task counter
+  MSM_ERR_HEAVY = 12,   // the number of heavy buckets
+  MSM_ERR_WORDS = 16,
+};
 
 #ifndef PCGPU_PAIR_MIN_BLOCKS
 #define PCGPU_PAIR_MIN_BLOCKS 4
@@ -633,38 +618,38 @@ int msm_reduce_launch(const MsmGeom &g, const uint32_t *task_off, const XYZZ<C> 
 
 // Runs the device pipeline on `st`.  d_scalars: n x 8 uint32 on the device.  On return (asynchronously)
 // *d_planes points at the S*c bit-plane sums, element (s*c + j) at index (s*c + j) * plane_stride, and
-// *d_err at a device word that is non-zero when a scalar was out of range.  `prof` brackets stages with events.
+// *d_err at the run's MSM_ERR_WORDS error words.  `prof` brackets stages with events.
 // *pair_threads / *pair_tdiv (if given) receive the pair-round kernel's thread count and wave divisor (0 without rounds).
 template <class C, class Prof>
 inline int msm_run(const uint32_t *tables, const MsmGeom &g, const uint32_t *d_scalars, rt::Arena &arena,
                    const XYZZ<C> **d_planes, size_t *plane_stride, uint32_t **d_err_out, rt::stream_t st, Prof &prof,
                    const uint32_t *pow2 = nullptr, uint32_t *pair_threads = nullptr, uint32_t *pair_tdiv = nullptr) {
-  int rc;
-  if ((rc = arena.reserve(msm_workspace_bytes<C>(g)))) return rc;
-  size_t max_entries = (size_t)g.n * g.W;
-  size_t max_tasks = max_entries / g.L + g.TB + 1;
-  uint32_t *counts = arena.take<uint32_t>(g.TB + 2);
-  uint32_t *offsets = arena.take<uint32_t>(g.TB + 2);
-  uint32_t *cursor = arena.take<uint32_t>(g.TB + 2);
-  uint32_t *ntasks = arena.take<uint32_t>(g.TB + 2);
-  uint32_t *task_off = arena.take<uint32_t>(g.TB + 2);
-  uint32_t *task_bucket = arena.take<uint32_t>(max_tasks);
-  uint32_t *entries = arena.take<uint32_t>(max_entries + 1);
-  uint32_t *scratch = arena.take<uint32_t>(scan_scratch_words(g.TB + 1));
-  uint32_t *err = arena.take<uint32_t>(16);  // err[0]: scalar out of range; err[8]: accumulate task queue
-  XYZZ<C> *partial = arena.take<XYZZ<C>>(max_tasks);
-  XYZZ<C> *buckets = arena.take<XYZZ<C>>(g.TB);
-  XYZZ<C> *planes = arena.take<XYZZ<C>>(msm_plane_scratch_elems(g));
-  XYZZ<C> *plane_out = arena.take<XYZZ<C>>((size_t)g.S * 2 * g.c);   // compact plane sums handed to the host
-  if (!counts || !offsets || !cursor || !ntasks || !task_off || !task_bucket || !entries || !scratch || !err || !partial ||
-      !buckets || !planes || !plane_out)
-    return rt::E_OOM;
+  using QF = Fp<typename C::Fq>;
+  const size_t max_entries = (size_t)g.n * g.W, max_tasks = max_entries / g.L + g.TB + 1;
+  const size_t bound0 = max_entries / 2 + g.TB + 1, bound1 = bound0 / 2 + g.TB + 1;   // pair-round output bounds
+  const bool pair_rounds = C::EXT == 1 && g.affine_rounds && pow2;   // G2 (C::EXT == 2) runs with R = 0: no pair-round kernels
+  uint32_t *counts, *offsets, *cursor, *ntasks, *task_off, *task_bucket, *entries, *scratch, *err;
+  XYZZ<C> *partial, *buckets, *planes, *plane_out;
+  uint32_t *offA = nullptr, *offB = nullptr, *cnt = nullptr, *src = nullptr;
+  QF *prefix = nullptr; Affine<C> *ptsA = nullptr, *ptsB = nullptr;
+  int rc = arena.carve([&](auto &&buf) {
+    buf(counts, g.TB + 2); buf(offsets, g.TB + 2); buf(cursor, g.TB + 2); buf(ntasks, g.TB + 2); buf(task_off, g.TB + 2);
+    buf(task_bucket, max_tasks); buf(entries, max_entries + 1); buf(scratch, scan_scratch_words(g.TB + 1)); buf(err, MSM_ERR_WORDS);
+    buf(partial, max_tasks); buf(buckets, g.TB); buf(planes, msm_plane_scratch_elems(g));
+    buf(plane_out, (size_t)g.S * 2 * g.c);   // compact plane sums handed to the host
+    if (pair_rounds) {
+      buf(offA, g.TB + 2); buf(offB, g.TB + 2); buf(cnt, g.TB + 2); buf(src, bound0);
+      buf(prefix, 3 * (bound0 + (1u << 20)));   // prefix | x1 | d  (x1, d: round 0 only)
+      buf(ptsA, bound0); buf(ptsB, bound1);
+    }
+  });
+  if (rc) return rc;
   *d_err_out = err; *d_planes = plane_out; *plane_stride = 1;
 
   prof.begin(0, st);
   if ((rc = rt::dev_memset(counts, 0, (g.TB + 2) * sizeof(uint32_t), st))) return rc;
-  if ((rc = rt::dev_memset(err, 0, 64, st))) return rc;
-  if ((rc = rt::launch<256>(MsmCountBody<C>{d_scalars, g, counts, err}, g.n, st))) return rc;
+  if ((rc = rt::dev_memset(err, 0, MSM_ERR_WORDS * sizeof(uint32_t), st))) return rc;
+  if ((rc = rt::launch<256>(MsmCountBody<C>{d_scalars, g, counts, err + MSM_ERR_RANGE}, g.n, st))) return rc;
   prof.end(0, st);
 
   prof.begin(1, st);
@@ -678,14 +663,7 @@ inline int msm_run(const uint32_t *tables, const MsmGeom &g, const uint32_t *d_s
 
   // ---- batched-affine pairwise rounds (msm_affine.cuh): halve every bucket g.affine_rounds times ----
   const Affine<C> *pts = nullptr;
-  if constexpr (C::EXT == 1) if (g.affine_rounds && pow2) {   // G2 (C::EXT == 2) runs with R = 0: no pair-round kernels
-    using QF = Fp<typename C::Fq>;
-    size_t bound0 = max_entries / 2 + g.TB + 1, bound1 = bound0 / 2 + g.TB + 1;
-    uint32_t *offA = arena.take<uint32_t>(g.TB + 2), *offB = arena.take<uint32_t>(g.TB + 2), *cnt = arena.take<uint32_t>(g.TB + 2);
-    uint32_t *src = arena.take<uint32_t>(bound0);
-    uint32_t *prefix = (uint32_t *)arena.take<QF>(3 * (bound0 + (1u << 20)));   // prefix | x1 | d  (x1, d: round 0 only)
-    Affine<C> *ptsA = arena.take<Affine<C>>(bound0), *ptsB = arena.take<Affine<C>>(bound1);
-    if (!offA || !offB || !cnt || !src || !prefix || !ptsA || !ptsB) return rt::E_OOM;
+  if constexpr (C::EXT == 1) if (pair_rounds) {
     size_t Tmax = 0;
     if ((rc = msm_pair_oneshot_threads<C>(&Tmax))) return rc;
     if (Tmax > (1u << 20)) Tmax = 1u << 20;
@@ -711,7 +689,7 @@ inline int msm_run(const uint32_t *tables, const MsmGeom &g, const uint32_t *d_s
       if ((rc = rt::launch<256>(PairPlanBody{off_in, off_out, g.TB, src}, bound, st))) return rc;
       uint32_t T = (uint32_t)Tmax;
       if (r == 0) prof.begin(12, st);
-      rc = msm_pair_round_oneshot<C>(r == 0, tables, g, entries, in, src, off_out, T, prefix, pow2, out, st);
+      rc = msm_pair_round_oneshot<C>(r == 0, tables, g, entries, in, src, off_out, T, (uint32_t *)prefix, pow2, out, st);
       if (rc) return rc;
       if (r == 0) prof.end(12, st);
       off_in = off_out;
@@ -722,18 +700,18 @@ inline int msm_run(const uint32_t *tables, const MsmGeom &g, const uint32_t *d_s
   }
 
   prof.begin(3, st);
-  if ((rc = rt::dev_memset(err + 12, 0, 4, st))) return rc;   // err[12]: number of heavy buckets; cursor[] is free again: heavy list
-  if ((rc = rt::launch<256>(TaskCountBody{offsets, g.L, ntasks, HEAVY_BUCKET_TASKS, err + 12, cursor}, g.TB, st))) return rc;
+  if ((rc = rt::dev_memset(err + MSM_ERR_HEAVY, 0, 4, st))) return rc;   // cursor[] is free again: heavy list
+  if ((rc = rt::launch<256>(TaskCountBody{offsets, g.L, ntasks, HEAVY_BUCKET_TASKS, err + MSM_ERR_HEAVY, cursor}, g.TB, st))) return rc;
   if ((rc = exclusive_scan_u32(ntasks, g.TB, task_off, scratch, st))) return rc;
   if ((rc = rt::launch<256>(TaskFillBody{task_off, task_bucket}, g.TB, st))) return rc;
   prof.end(3, st);
 
   prof.begin(4, st);
-  if ((rc = msm_accumulate_launch<C>(tables, g, offsets, task_off, task_bucket, entries, partial, err + 8, pts, st))) return rc;
+  if ((rc = msm_accumulate_launch<C>(tables, g, offsets, task_off, task_bucket, entries, partial, err + MSM_ERR_QUEUE, pts, st))) return rc;
   prof.end(4, st);
 
   prof.begin(5, st);
-  if ((rc = msm_reduce_launch<C>(g, task_off, partial, buckets, planes, plane_out, err + 12, cursor, st))) return rc;
+  if ((rc = msm_reduce_launch<C>(g, task_off, partial, buckets, planes, plane_out, err + MSM_ERR_HEAVY, cursor, st))) return rc;
   prof.end(5, st);
   return rt::OK;
 }

@@ -12,6 +12,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include <atomic>
+#include <type_traits>
 
 #ifndef PCGPU_EMUL
 #include <cuda_runtime.h>
@@ -243,28 +244,36 @@ template <class T> __device__ __forceinline__ T atomic_or(T *p, T v) { return at
 #define PCGPU_KERNEL_DEV __device__ __forceinline__
 #endif
 
-// Bump allocator over one device arena (re-used across calls; grown on demand).
+// One device arena, re-used across calls and grown on demand, laid out afresh by every carve().
 struct Arena {
   char *base = nullptr;
-  size_t cap = 0, used = 0;
+  size_t cap = 0;
   int reserve(size_t bytes) {
-    if (bytes <= cap) { used = 0; return OK; }
+    if (bytes <= cap) return OK;
     if (base) dev_free(base);
-    base = nullptr; cap = 0; used = 0;
+    base = nullptr; cap = 0;
     int rc = dev_malloc((void **)&base, bytes);
     if (rc) return rc;
     cap = bytes;
     return OK;
   }
-  template <class T> T *take(size_t count) {
-    size_t bytes = (count * sizeof(T) + 255) & ~(size_t)255;
-    if (used + bytes > cap) return nullptr;
-    T *p = (T *)(base + used);
-    used += bytes;
-    return p;
+  // Lays the arena out as the buffers `list` names.  list(buf) calls buf(p, count) once per buffer, in layout order, with p a
+  // T *& and count its elements; it runs twice, once to reserve the sum and once to point every p at its buffer.  Each buffer
+  // takes whole 256-byte granules, at least one, so a zero-length buffer still gets a valid, distinct pointer.
+  template <class List> int carve(const List &list) {
+    size_t used = 0;
+    list([&](auto *&p, size_t count) { used += padded(sizeof *p, count); });
+    int rc = reserve(used);
+    if (rc) return rc;
+    used = 0;
+    list([&](auto *&p, size_t count) {
+      p = reinterpret_cast<std::remove_reference_t<decltype(p)>>(base + used);
+      used += padded(sizeof *p, count);
+    });
+    return OK;
   }
-  static size_t pad(size_t bytes) { return (bytes + 255) & ~(size_t)255; }
-  void release() { if (base) dev_free(base); base = nullptr; cap = used = 0; }
+  static size_t padded(size_t elem, size_t count) { size_t b = elem * count; return ((b ? b : 1) + 255) & ~(size_t)255; }
+  void release() { if (base) dev_free(base); base = nullptr; cap = 0; }
 };
 
 }  // namespace rt

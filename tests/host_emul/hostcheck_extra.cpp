@@ -9,7 +9,7 @@ using namespace pcgpu;
 template <class P>
 static const uint32_t *pow2_table() {
   static std::vector<uint32_t> t;
-  if (t.empty()) { t.resize((64 * P::N + 1) * P::N); Pow2TableBody<P>{t.data()}(0); }
+  if (t.empty()) { t.resize(pow2_table_bytes<P>() / 4); Pow2TableBody<P>{t.data()}(0); }
   return t.data();
 }
 

@@ -605,13 +605,14 @@ def oracle_ipa_rounds(cname, comm_key, coeffs, point, h_prime, round_challenge):
         def cm(keypart, sc, ip):
             msm, inf = orc.msm(C.id, keypart, orc.field_unop("orc_fr_from_mont", C.id, sc))
             hp, hinf = orc.g1_mul(C.id, h_prime, orc.field_unop("orc_fr_from_mont", C.id, ip.reshape(1, 4)))
-            return orc.g1_sum(C.id, np.stack([msm, hp]), inf=np.array([inf, hinf], dtype=np.uint8))[0]
-        l = cm(key[:m], co[m:n], orc.fr_inner_product(C.id, co[m:n], z[:m]))
-        r = cm(key[m:n], co[:m], orc.fr_inner_product(C.id, co[:m], z[m:n]))
+            return orc.g1_sum(C.id, np.stack([msm, hp]), inf=np.array([inf, hinf], dtype=np.uint8))
+        l, l_inf = cm(key[:m], co[m:n], orc.fr_inner_product(C.id, co[m:n], z[:m]))
+        r, r_inf = cm(key[m:n], co[:m], orc.fr_inner_product(C.id, co[:m], z[m:n]))
         l_vec.append(l); r_vec.append(r)
         # the reference's transcript, built independently of the device encoder: canonical LE scalar, then ark-serialize's
-        # uncompressed encodings of l and r (oracle/pyref.py)
-        data = int(round_challenge).to_bytes(32, "little") + pyref.g1_serialize(C, C.points_from_limbs(np.stack([l, r])), False)
+        # uncompressed encodings of l and r (oracle/pyref.py; an identity l or r carries the infinity flag)
+        pts = C.points_from_limbs(np.stack([l, r]), inf=[l_inf, r_inf])
+        data = int(round_challenge).to_bytes(32, "little") + pyref.g1_serialize(C, pts, False)
         digest_i = 0
         while True:                                                   # compute_random_oracle_challenge, ipa_pc/mod.rs:74-87
             import hashlib
@@ -628,7 +629,8 @@ def oracle_ipa_rounds(cname, comm_key, coeffs, point, h_prime, round_challenge):
     return dict(l_vec=l_vec, r_vec=r_vec, final_comm_key=key[0], c=co[0])
 
 
-@pytest.mark.parametrize("cname,n", [("pallas", 64), ("bls12_381", 16), ("bn254", 32)])
+@pytest.mark.parametrize("cname,n", [("pallas", 64), ("bls12_381", 16), ("bn254", 32),
+                                     ("bls12_381", 4), ("pallas", 8)])   # Fr vectors below / at one 256-byte arena granule
 def test_ipa_open_rounds(eng, pc, cname, n, msm_path):
     """cfg3's dataflow (Pallas; the reference instantiates IPA on Jubjub only): every l, r, the final key and c."""
     from poly_commit_b200 import ipa_pc
