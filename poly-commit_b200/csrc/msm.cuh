@@ -295,7 +295,7 @@ PCGPU_DEV Affine<C> load_affine(const Affine<C> *p) {
 
 // Table records: x at word 0, y at word g.y_words, record stride g.pt_words.  The window-folded BLS12-381 tables use
 // 128-byte records (x in the first 64-byte half, y in the second) so that an x-only read is ONE aligned 64-byte DRAM
-// access and a full read two; raw base arrays keep the ABI's packed x||y.
+// access and a full read one aligned 128-byte line; raw base arrays keep the ABI's packed x||y.
 template <class C>
 PCGPU_DEV const uint32_t *table_record(const uint32_t *tables, size_t idx, const MsmGeom &g) { return tables + idx * g.pt_words; }
 template <class C>
@@ -639,7 +639,7 @@ inline int msm_run(const uint32_t *tables, const MsmGeom &g, const uint32_t *d_s
     buf(plane_out, (size_t)g.S * 2 * g.c);   // compact plane sums handed to the host
     if (pair_rounds) {
       buf(offA, g.TB + 2); buf(offB, g.TB + 2); buf(cnt, g.TB + 2); buf(src, bound0);
-      buf(prefix, 3 * (bound0 + (1u << 20)));   // prefix | x1 | d  (x1, d: round 0 only)
+      buf(prefix, bound0 + (1u << 20));   // prefix products: slots rounded up to whole waves of T <= 2^20 threads
       buf(ptsA, bound0); buf(ptsB, bound1);
     }
   });

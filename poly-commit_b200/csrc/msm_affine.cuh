@@ -11,7 +11,8 @@
 // t, t+T, t+2T, ... (coalesced); pass 1 walks them accumulating the running product of the denominators
 // (x2 - x1) and storing the prefix products, pass 2 walks back turning the single inverse into every 1/(x2 - x1)
 // and emitting the sums.  Exceptional pairs (P = Q, P = -Q, identity operands) get denominator 2y / 1 and are
-// resolved in pass 2.  After R rounds the remaining points (a few per bucket) go through the XYZZ task kernel.
+// resolved in pass 2.  Round 0 reads its operands from the window-folded tables: the x halves of the records in pass 1, the
+// whole records in pass 2.  After R rounds the remaining points (a few per bucket) go through the XYZZ task kernel.
 #pragma once
 #include "msm.cuh"
 
@@ -94,7 +95,7 @@ struct MsmAffinePairBody {
   const Affine<C> *pts_in;                                      // later rounds: operands are affine points
   uint32_t *src; const uint32_t *off_out;                       // plan; total outputs = off_out[g.TB] (pass 1 may set PAIR_EXC)
   uint32_t T;                                                   // threads in this launch
-  uint32_t *prefix;                                             // per (iteration, thread): prefix product; round 0 also x1 and d
+  uint32_t *prefix;                                             // per (iteration, thread): prefix product
   const uint32_t *pow2;                                         // fp_inv_gcd table
   Affine<C> *pts_out;
 
@@ -146,8 +147,6 @@ struct MsmAffinePairBody {
     constexpr int N = Q::N;
     if (t >= T) return;
     const uint32_t total = off_out[g.TB];
-    uint32_t *xbuf = prefix + (size_t)T * N * ((total + T - 1) / T);   // round 0 only: x1 per slot, then d per slot
-    uint32_t *dbuf = xbuf + (size_t)T * N * ((total + T - 1) / T);
     // ---- pass 1: running product of the denominators, prefix products to memory ----
     const uint32_t kmax = (uint32_t)t < total ? (total - (uint32_t)t + T - 1) / T : 0u;   // slots k*T + t < total
     Fp<Q> acc = Fp<Q>::one();
@@ -159,9 +158,9 @@ struct MsmAffinePairBody {
         if (k + 1 < kmax) nxt = fetch_slot((k + 1) * T + (uint32_t)t);   // descriptor of the next slot: in flight during this one
         Fp<Q> d;
         if (FROM_TABLES) {
-          // Round 0 gathers every base twice (x here, y in pass 2).  x1 and the denominator are written out next to the
-          // prefix product (coalesced), so pass 2 re-reads them sequentially and gathers ONLY the y halves of the records:
-          // the random traffic of the round halves (random 64/128-byte HBM accesses run at ~1/4 of the streaming rate).
+          // Round 0 reads x here (the first 64-byte half of each record) and the whole record in pass 2.  On H100 a random
+          // 128-byte access costs about what a random 64-byte one does, so pass 2 gets x back with y in the same access
+          // instead of re-reading a spilled x1 and d: only the prefix product goes through memory.
           Fp<Q> x1 = slot_x(cur, 0);
           bool exc = false;
           if (cur.b == PAIR_NONE) d = Fp<Q>::one();
@@ -171,8 +170,6 @@ struct MsmAffinePairBody {
             else { Affine<C> P = slot_point(cur, 0), Qp = slot_point(cur, 1); pair_classify<C>(P, Qp, false, d); exc = true; }
           }
           if (exc) src[k * T + (uint32_t)t] |= PAIR_EXC;
-          store_fq<Q>(xbuf + ((size_t)k * T + t) * N, x1);
-          store_fq<Q>(dbuf + ((size_t)k * T + t) * N, d);
         } else {
           d = slot_denominator(cur);
         }
@@ -192,20 +189,18 @@ struct MsmAffinePairBody {
       if (k > 0) nxt2 = fetch_slot(o - T);
       bool single = cur.b == PAIR_NONE;
       if (FROM_TABLES && !exc) {
-        // fast path: x1, d from pass 1 (sequential), y halves gathered
-        Fp<Q> x1 = load_fq<Q>(xbuf + ((size_t)k * T + t) * N), d = load_fq<Q>(dbuf + ((size_t)k * T + t) * N);
-        Fp<Q> y1 = fp_cneg<Q>(load_fq<Q>(slot_rec(cur.a) + g.y_words), (cur.a & ENTRY_SIGN) != 0);
+        // fast path: whole records gathered (an ordinary pair or a single), d recomputed from the two x
+        Affine<C> P = slot_point(cur, 0), Qp = P;
+        if (!single) Qp = slot_point(cur, 1);
+        Fp<Q> d = single ? Fp<Q>::one() : fp_sub<Q>(Qp.x, P.x);
         Fp<Q> dinv = fp_mul<Q>(inv, load_fq<Q>(prefix + ((size_t)k * T + t) * N));
         inv = fp_mul<Q>(inv, d);
-        Affine<C> R;
-        if (single) { R.x = x1; R.y = y1; if (x1.is_zero() && y1.is_zero()) R = Affine<C>::inf(); }
-        else {
-          Fp<Q> y2 = fp_cneg<Q>(load_fq<Q>(slot_rec(cur.b) + g.y_words), (cur.b & ENTRY_SIGN) != 0);
-          Fp<Q> lam = fp_mul<Q>(fp_sub<Q>(y2, y1), dinv);
-          Fp<Q> x2 = fp_add<Q>(x1, d);
-          Fp<Q> x3 = fp_sub<Q>(fp_sub<Q>(fp_sqr<Q>(lam), x1), x2);
+        Affine<C> R = P;   // a single: P itself (the identity record is (0, 0))
+        if (!single) {
+          Fp<Q> lam = fp_mul<Q>(fp_sub<Q>(Qp.y, P.y), dinv);
+          Fp<Q> x3 = fp_sub<Q>(fp_sub<Q>(fp_sqr<Q>(lam), P.x), Qp.x);
           R.x = x3;
-          R.y = fp_sub<Q>(fp_mul<Q>(lam, fp_sub<Q>(x1, x3)), y1);
+          R.y = fp_sub<Q>(fp_mul<Q>(lam, fp_sub<Q>(P.x, x3)), P.y);
         }
         Affine<C> *dst0 = pts_out + o;
         store_fq<Q>(reinterpret_cast<uint32_t *>(dst0), R.x);
