@@ -392,7 +392,7 @@ int pcgpu_measure_imad_peak(pcgpu_ctx *ctx, double *ops_per_s);
 /* Kernels launched by this library in the calling process so far (bench.py's gpu_launches). */
 uint64_t pcgpu_launch_count(void);
 int pcgpu_selftest_field(pcgpu_ctx *ctx, int curve, uint64_t seed, size_t n, uint64_t *mismatches);
-/* The path and geometry the context's most recent MSM took, each value recorded where the library decided it.  Writes
+/* The path and geometry the context's most recent MSM took, each value taken from the MSM's plan.  Writes
  * min(len, PCGPU_GEOM_FIELDS) words: out[PCGPU_GEOM_PATH] is PCGPU_MSM_PATH_NONE (n = 0, or no MSM yet), _SMALL (one-launch
  * kernel; out[PCGPU_GEOM_SPLIT] = blocks per window: 1, 3 or 6) or _BUCKETS (the bucket pipeline: window bits c, windows W,
  * table groups G (1 = raw bases), batched-affine rounds R, the pair-round kernel's threads T and its divisor tdiv, the one

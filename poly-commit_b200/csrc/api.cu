@@ -80,8 +80,8 @@ extern "C" int pcgpu_init(int device, pcgpu_ctx **out) {
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return PCGPU_E_CUDA;
   if (prop.major != 9 || prop.minor != 0) return PCGPU_E_CUDA;  // built for sm_90a only; no other code path exists
   if (cudaSetDevice(device) != cudaSuccess) return PCGPU_E_CUDA;
-  // L2 fetch granularity hint: the table gathers of the pair rounds read ONE 64-byte half record (x in pass 1, y in pass 2)
-  // per access; at the default granularity every such miss moves a whole 128-byte line from DRAM.
+  // L2 fetch granularity hint: round 0 of the pair rounds gathers the 64-byte x halves of table records in pass 1 and whole
+  // 128-byte records in pass 2 (DESIGN.md section 5); at the default granularity every pass-1 miss moves a 128-byte line.
   if (const char *e = getenv("PCGPU_L2_FETCH_GRANULARITY")) {
     int v = atoi(e);
     if (v == 32 || v == 64 || v == 128) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)v);

@@ -191,15 +191,6 @@ template <class R> inline void fr_from_mont_host(const void *in, uint64_t *out) 
   HFp<R> r = mul<R>(a, one); memcpy(out, r.l, sizeof r.l);
 }
 
-// Combination of the device's bit-plane sums T[s][j] = sum of the buckets of set s whose weight has bit j set:
-//   result = sum_s 2^(c s) * sum_j 2^j T[s][j]
-template <class C> inline HXYZZ<C> combine_bit_planes(const HXYZZ<C> *T, uint32_t S, uint32_t c) {
-  // plane j of set s carries weight 2^(c s + j): one Horner pass over the bit positions, S*c doublings and additions
-  HXYZZ<C> acc = HXYZZ<C>::inf();
-  for (uint32_t b = S * c; b-- > 0;) { acc = pdbl<C>(acc); acc = padd<C>(acc, T[b]); }
-  return acc;
-}
-
 // Small-MSM path (msm_small.cuh): the device hands back one point per window, U_w = sum_k k B_{w,k};
 //   result = sum_w 2^(c w) U_w   -- c * (W - 1) doublings and W additions
 template <class C> inline HXYZZ<C> combine_windows(const HXYZZ<C> *U, uint32_t W, uint32_t c) {
@@ -211,8 +202,10 @@ template <class C> inline HXYZZ<C> combine_windows(const HXYZZ<C> *U, uint32_t W
   return acc;
 }
 
-// Two-level variant (large windows): per set the device hands back the planes of the column sums C (weights lo+1, bits_c
-// of them) followed by the planes of the row sums R (weights hi, bits_r):  set value = sum_j 2^j TC_j + 2^h * sum_j 2^j TR_j
+// Combination of the device's bit-plane sums (msm.cuh, two-level reduction): per set the device hands back the planes of the
+// column sums C (weights lo+1, bits_c of them) followed by the planes of the row sums R (weights hi, bits_r):
+//   set value = sum_j 2^j TC_j + 2^h * sum_j 2^j TR_j,   result = sum_s 2^(c s) * set value
+// (S = c = 1, h = 0: the one plane itself -- the peer path's one-point record)
 template <class C> inline HXYZZ<C> combine_bit_planes_2level(const HXYZZ<C> *T, uint32_t S, uint32_t c, uint32_t h) {
   const uint32_t bits_c = h + 1, bits_r = c - 1 - h, per = bits_c + bits_r;
   HXYZZ<C> acc = HXYZZ<C>::inf();

@@ -99,7 +99,7 @@ struct pcgpu_ctx {
   rt::Arena msm_arena, stage;
   rt::Arena ipa_arena;             // state of the (one) InnerProductArgPC::open in progress on this context; reused across opens
   bool ipa_active = false;
-  uint32_t pair_tdiv = 1;          // set by the batch entry points while several pipelines are in flight (msm_run)
+  uint32_t pair_tdiv = 1;          // set by the batch entry points while several pipelines are in flight (msm_plan)
   DeviceWords *d_words = nullptr;
   Prof prof;
   uint32_t *d_pow2[3] = {nullptr, nullptr, nullptr};  // fp_inv_gcd tables (Fq), per curve
@@ -229,6 +229,13 @@ inline uint32_t comb_window_bits(size_t n, size_t point_bytes) {
   return best;
 }
 
+// the comb tables of n bases with c-bit windows (srs.cuh): W windows of NBk entries per base; the row fields are left 0
+template <class C> inline CombGeom comb_geometry(size_t n_bases, uint32_t c) {
+  CombGeom g{};
+  g.n_bases = (uint32_t)n_bases; g.c = c; g.W = (C::Fr::BITS + c - 1) / c; g.NBk = 1u << (c - 1);
+  return g;
+}
+
 template <class C>
 int srs_register_impl(pcgpu_ctx *ctx, const void *bases, const uint8_t *inf, size_t n, uint32_t flags, pcgpu_srs *srs) {
   const size_t psz = sizeof(Affine<C>);
@@ -256,8 +263,7 @@ int srs_register_impl(pcgpu_ctx *ctx, const void *bases, const uint8_t *inf, siz
     if constexpr (C::EXT == 1) {
     if (groups > 1 && (rc = srs_build_groups<C>((const Affine<C> *)srs->d_tables, (uint32_t *)srs->d_folded, n, c, groups, st))) return rc;
     if (flags & PCGPU_SRS_COMB) {
-      CombGeom cg; memset(&cg, 0, sizeof cg);
-      cg.n_bases = (uint32_t)n; cg.c = comb_window_bits(n, psz); cg.W = (C::Fr::BITS + cg.c - 1) / cg.c; cg.NBk = 1u << (cg.c - 1);
+      const CombGeom cg = comb_geometry<C>(n, comb_window_bits(n, psz));
       if ((rc = rt::dev_malloc(&srs->d_comb, psz * n * cg.W * cg.NBk))) return rc;
       srs->comb_c = cg.c;
       if ((rc = ensure_pow2<C>(ctx))) return rc;
@@ -283,21 +289,87 @@ inline bool msm_small_enabled() {
   const char *e = getenv("PCGPU_MSM_SMALL");
   return !(e && e[0] == '0');
 }
+
+// The small-path plan for problems of at most nmax terms.  Blocks per window: 1 below 512 terms, 3 up to SMALL_MAX_N, 6 beyond
+// (the IPA's l / r commitments of 8192 terms: a block's share stays at <= 1366 terms, which is what bounds its chain of
+// dependent additions and its digit buffer)
+inline MsmPlan msm_small_plan(size_t nmax) {
+  return MsmPlan{PCGPU_MSM_PATH_SMALL, nmax, (uint32_t)(nmax > SMALL_MAX_N ? 2 * SMALL_SPLIT : nmax >= SMALL_SPLIT_MIN_N ? SMALL_SPLIT : 1)};
+}
+
+// Decides how one MSM of n terms over srs's bases from base_offset runs: the path, and for the bucket pipeline the tables, the
+// window, the task length and the batched-affine pair rounds.  The tuning knobs are read here, on every call.
 template <class C>
-int msm_small_to_host(pcgpu_ctx *ctx, const MsmSmallProblem<C> *probs, uint32_t nprob, bool mont, host::HXYZZ<C> *out) {
+int msm_plan(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, size_t n, bool mont, MsmPlan *p) {
+  *p = MsmPlan{};
+  if (n == 0) return PCGPU_OK;
+  if (n <= SMALL_MAX_N && msm_small_enabled()) { *p = msm_small_plan(n); return PCGPU_OK; }
+  p->path = PCGPU_MSM_PATH_BUCKETS; p->n = n;
+  const bool folded = srs->groups > 1 && n >= SRS_PRECOMPUTE_MIN_N;   // window-folded tables, one group per window
+  p->tables = (const uint32_t *)(folded ? srs->d_folded : srs->d_tables);
+  uint32_t c = folded ? srs->c : msm_pick_c(n), L = 32;
+  if (!folded) if (const char *e = getenv("PCGPU_MSM_C")) { int v = atoi(e); if (v >= 8 && v <= 22) c = (uint32_t)v; }   // tuning / test knob
+  if (const char *e = getenv("PCGPU_MSM_L")) { int v = atoi(e); if (v >= 4 && v <= 4096) L = (uint32_t)v; }   // tuning knob
+  MsmGeom &g = p->g;
+  g = msm_geometry(n, c, folded ? srs->groups : 1, C::Fr::BITS, mont, srs->n, base_offset, L);
+  g.pt_words = folded ? aligned_pt_words<C>() : 2 * coord_words<typename C::F>();
+  g.y_words = folded ? aligned_y_words<C>() : coord_words<typename C::F>();
+  if constexpr (C::EXT == 1) {   // G2: no batched-affine rounds (R = 0)
+    if (int rc = msm_pair_oneshot_threads<C>(&p->wave)) return rc;
+    // batched-affine rounds while buckets hold >= 64 points and a round still gives every thread >= 16 additions
+    const size_t entries = (size_t)g.n * g.W, avg = entries / g.TB, wave = p->wave;
+    uint32_t R = 0;
+    while (R < 8 && (avg >> R) >= 4 && (entries >> (R + 1)) >= 16 * wave) R++;
+    if (const char *e = getenv("PCGPU_MSM_AFFINE_ROUNDS")) { int v = atoi(e); if (v >= 0 && v <= 12) R = (uint32_t)v; }
+    g.affine_rounds = R;
+    if (R) {
+      // Throughput mode (several MSM pipelines in flight on sibling streams): half a wave per pair kernel, so that the pair
+      // kernels of TWO pipelines are co-resident on every SM -- a full wave owns the whole register file -- and the DRAM-bound
+      // pass 1 and the ALU-bound inversion of one overlap the multiply-bound pass 2 of the other; every thread then covers
+      // twice the slots with the same single inversion per round.
+      uint32_t tdiv = ctx->pair_tdiv ? ctx->pair_tdiv : 1;
+      if (const char *e = getenv("PCGPU_MSM_AFFINE_TDIV")) { int v = atoi(e); if (v >= 1 && v <= 16) tdiv = (uint32_t)v; }  // tuning knob
+      size_t T = wave < (1u << 20) ? wave : (1u << 20);
+      if (tdiv > 1) T = (T / tdiv + 127) / 128 * 128;
+      g.pair_tdiv = tdiv; p->T = (uint32_t)T;
+    }
+  }
+  return PCGPU_OK;
+}
+
+// pcgpu_msm_last_geometry's words for the MSM `p` plans; msm_collect adds the heavy-bucket count once the pipeline has run
+inline void msm_report(pcgpu_ctx *ctx, const MsmPlan &p) {
+  uint64_t *lg = ctx->last_geom;
+  memset(lg, 0, sizeof ctx->last_geom);
+  lg[PCGPU_GEOM_PATH] = p.path; lg[PCGPU_GEOM_SPLIT] = p.split; lg[PCGPU_GEOM_N] = p.n;
+  if (p.path != PCGPU_MSM_PATH_BUCKETS) return;
+  const MsmGeom &g = p.g;
+  lg[PCGPU_GEOM_C] = g.c; lg[PCGPU_GEOM_W] = g.W; lg[PCGPU_GEOM_G] = g.G; lg[PCGPU_GEOM_R] = g.affine_rounds;
+  lg[PCGPU_GEOM_T] = p.T; lg[PCGPU_GEOM_TDIV] = g.pair_tdiv; lg[PCGPU_GEOM_WAVE] = p.wave;
+  lg[PCGPU_GEOM_ENTRIES] = (uint64_t)g.n * g.W;
+  lg[PCGPU_GEOM_HEAVY] = UINT64_MAX;
+}
+
+// the same for a pcgpu_msm_batch over comb tables
+inline void comb_report(pcgpu_ctx *ctx, const CombGeom &g) {
+  uint64_t *lg = ctx->last_geom;
+  memset(lg, 0, sizeof ctx->last_geom);
+  lg[PCGPU_GEOM_PATH] = PCGPU_MSM_PATH_COMB; lg[PCGPU_GEOM_N] = g.n; lg[PCGPU_GEOM_C] = g.c; lg[PCGPU_GEOM_W] = g.W;
+  lg[PCGPU_GEOM_SPLIT] = g.seg_len; lg[PCGPU_GEOM_ENTRIES] = (uint64_t)g.count * g.segs;
+}
+
+// Runs the small-path plan p over nprob problems of at most p.n terms each.
+template <class C>
+int msm_small_to_host(pcgpu_ctx *ctx, const MsmPlan &p, const MsmSmallProblem<C> *probs, uint32_t nprob, bool mont,
+                      host::HXYZZ<C> *out) {
   using R = typename C::Fr;
   constexpr uint32_t W = small_windows<R>();
   rt::stream_t st = ctx->stream;
   int rc;
-  if (nprob == 0 || nprob > SMALL_MAX_PROB) return PCGPU_E_BADARG;
-  uint32_t nmax = 0;
-  for (uint32_t p = 0; p < nprob; p++) nmax = probs[p].n > nmax ? probs[p].n : nmax;
-  // blocks per window: 1 below 512 terms, 3 up to SMALL_MAX_N, 6 beyond (the IPA's l / r commitments of 8192 terms: a block's
-  // share stays at <= 1366 terms, which is what bounds its chain of dependent additions and its digit buffer)
-  if (nmax > 2 * SMALL_MAX_N) return PCGPU_E_BADARG;
-  const uint32_t split = nmax > SMALL_MAX_N ? 2 * SMALL_SPLIT : (nmax >= SMALL_SPLIT_MIN_N ? SMALL_SPLIT : 1);
-  memset(ctx->last_geom, 0, sizeof ctx->last_geom);
-  ctx->last_geom[PCGPU_GEOM_PATH] = PCGPU_MSM_PATH_SMALL; ctx->last_geom[PCGPU_GEOM_SPLIT] = split; ctx->last_geom[PCGPU_GEOM_N] = nmax;
+  if (p.path != PCGPU_MSM_PATH_SMALL || p.n > 2 * SMALL_MAX_N || nprob == 0 || nprob > SMALL_MAX_PROB) return PCGPU_E_BADARG;
+  for (uint32_t i = 0; i < nprob; i++) if (probs[i].n > p.n) return PCGPU_E_BADARG;
+  msm_report(ctx, p);
+  const uint32_t split = p.split;   // blocks per window
   const size_t npts = (size_t)nprob * W * split;
   uint32_t *d_err; XYZZ<C> *d_out;
   if ((rc = ctx->msm_arena.carve([&](auto &&buf) { buf(d_err, 1); buf(d_out, npts); }))) return rc;
@@ -331,48 +403,14 @@ int msm_small_to_host(pcgpu_ctx *ctx, const MsmSmallProblem<C> *probs, uint32_t 
   return PCGPU_OK;
 }
 
-// Device half of one bucket-pipeline MSM (n > SMALL_MAX_N or the small path disabled): picks the geometry, runs msm_run on
-// the context's stream and returns (asynchronously) the compact S*c bit-plane sums and the error words.
+// Device half of a bucket-pipeline plan: runs msm_run on the context's stream and returns (asynchronously) the packed S*c
+// bit-plane sums and the error words.
 template <class C>
-int msm_device_planes(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, const uint32_t *d_scalars, size_t n,
-                             bool mont, MsmGeom *g_out, const XYZZ<C> **d_planes, size_t *stride, uint32_t **d_err) {
-  rt::stream_t st = ctx->stream;
-  uint32_t c, groups;
-  const uint32_t *tables = (const uint32_t *)srs->d_tables;
-  uint32_t pt_words = 2 * coord_words<typename C::F>(), y_words = coord_words<typename C::F>();
-  if (srs->groups > 1 && n >= SRS_PRECOMPUTE_MIN_N) {
-    c = srs->c; groups = srs->groups;
-    tables = (const uint32_t *)srs->d_folded; pt_words = aligned_pt_words<C>(); y_words = aligned_y_words<C>();
-  } else {
-    c = msm_pick_c(n); groups = 1;
-    if (const char *e = getenv("PCGPU_MSM_C")) { int v = atoi(e); if (v >= 8 && v <= 22) c = (uint32_t)v; }   // tuning / test knob
-  }
-  MsmGeom g = msm_geometry(n, c, groups, C::Fr::BITS, mont, srs->n, base_offset);
-  g.pt_words = pt_words; g.y_words = y_words; g.pair_tdiv = ctx->pair_tdiv;
+int msm_device_planes(pcgpu_ctx *ctx, const MsmPlan &p, const uint32_t *d_scalars, const XYZZ<C> **d_planes, uint32_t **d_err) {
+  msm_report(ctx, p);
   int rc;
-  // batched-affine rounds while buckets hold >= 64 points and a round still gives every thread >= 16 additions
-  {
-    size_t Tmax = 0, entries = (size_t)g.n * g.W;
-    uint32_t R = 0;
-    if constexpr (C::EXT == 1) {   // G2: no batched-affine rounds (R = 0)
-      if ((rc = msm_pair_oneshot_threads<C>(&Tmax))) return rc;
-      size_t avg = entries / g.TB;
-      while (R < 8 && (avg >> R) >= 4 && (entries >> (R + 1)) >= 16 * Tmax) R++;
-      if (const char *e = getenv("PCGPU_MSM_AFFINE_ROUNDS")) { int v = atoi(e); if (v >= 0 && v <= 12) R = (uint32_t)v; }
-    }
-    g.affine_rounds = R;
-    uint64_t *lg = ctx->last_geom;
-    memset(lg, 0, sizeof ctx->last_geom);
-    lg[PCGPU_GEOM_PATH] = PCGPU_MSM_PATH_BUCKETS; lg[PCGPU_GEOM_N] = g.n; lg[PCGPU_GEOM_C] = g.c; lg[PCGPU_GEOM_W] = g.W;
-    lg[PCGPU_GEOM_G] = g.G; lg[PCGPU_GEOM_R] = R; lg[PCGPU_GEOM_WAVE] = Tmax; lg[PCGPU_GEOM_ENTRIES] = entries;
-    lg[PCGPU_GEOM_HEAVY] = UINT64_MAX;   // msm_collect fills it in from the pipeline's error words
-  }
-  if (g.affine_rounds && (rc = ensure_pow2<C>(ctx))) return rc;
-  *g_out = g;
-  uint32_t T = 0, tdiv = 0;
-  rc = msm_run<C>(tables, g, d_scalars, ctx->msm_arena, d_planes, stride, d_err, st, ctx->prof, ctx->d_pow2[C::ID], &T, &tdiv);
-  ctx->last_geom[PCGPU_GEOM_T] = T; ctx->last_geom[PCGPU_GEOM_TDIV] = tdiv;
-  return rc;
+  if (p.g.affine_rounds && (rc = ensure_pow2<C>(ctx))) return rc;
+  return msm_run<C>(p, d_scalars, ctx->msm_arena, d_planes, d_err, ctx->stream, ctx->prof, ctx->d_pow2[C::ID]);
 }
 
 // One MSM in two halves so that a caller can keep several pipelines in flight from one host thread:
@@ -385,28 +423,30 @@ struct MsmPending {
   bool done = true;            // result already in `ready`
   host::HXYZZ<C> ready;
   MsmGeom g;
-  size_t np = 0;
 };
 
 template <class C>
 int msm_issue(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, const uint32_t *d_scalars, size_t n, bool mont,
               MsmPending<C> *p) {
   rt::stream_t st = ctx->stream;
-  p->done = true; p->ready = host::HXYZZ<C>::inf(); p->np = 0;
-  if (n == 0) { memset(ctx->last_geom, 0, sizeof ctx->last_geom); return PCGPU_OK; }
-  if (n <= SMALL_MAX_N && msm_small_enabled()) {
-    MsmSmallProblem<C> pr{(const Affine<C> *)srs->d_tables + base_offset, d_scalars, nullptr, nullptr, (uint32_t)n};
-    return msm_small_to_host<C>(ctx, &pr, 1, mont, &p->ready);
-  }
-  const XYZZ<C> *d_planes = nullptr; size_t stride = 0; uint32_t *d_err = nullptr;
-  int rc = msm_device_planes<C>(ctx, srs, base_offset, d_scalars, n, mont, &p->g, &d_planes, &stride, &d_err);
+  p->done = true; p->ready = host::HXYZZ<C>::inf();
+  MsmPlan plan;
+  int rc = msm_plan<C>(ctx, srs, base_offset, n, mont, &plan);
   if (rc) return rc;
-  p->np = (size_t)p->g.S * p->g.c;   // one-level: c planes per set; two-level: (h+1) + (c-1-h) = c planes per set as well
+  if (plan.path == PCGPU_MSM_PATH_NONE) { msm_report(ctx, plan); return PCGPU_OK; }
+  if (plan.path == PCGPU_MSM_PATH_SMALL) {
+    MsmSmallProblem<C> pr{(const Affine<C> *)srs->d_tables + base_offset, d_scalars, nullptr, nullptr, (uint32_t)n};
+    return msm_small_to_host<C>(ctx, plan, &pr, 1, mont, &p->ready);
+  }
+  const XYZZ<C> *d_planes = nullptr; uint32_t *d_err = nullptr;
+  if ((rc = msm_device_planes<C>(ctx, plan, d_scalars, &d_planes, &d_err))) return rc;
+  p->g = plan.g;
+  const size_t np = (size_t)p->g.S * p->g.c;   // (h+1) + (c-1-h) = c planes per set
   static_assert(sizeof(host::HXYZZ<C>) == sizeof(XYZZ<C>), "host/device point layouts must agree");
   static_assert(PCGPU_MAX_PLANES * sizeof(XYZZ<C>) <= sizeof(PinnedZone::planes), "the plane sums must fit the pinned zone");
-  if (p->np > PCGPU_MAX_PLANES || !ctx->h_pinned) return PCGPU_E_BADARG;
+  if (np > PCGPU_MAX_PLANES || !ctx->h_pinned) return PCGPU_E_BADARG;
   PinnedZone *hp = ctx->h_pinned;
-  if ((rc = rt::copy_d2h_2d(hp->planes, sizeof(XYZZ<C>), d_planes, stride * sizeof(XYZZ<C>), sizeof(XYZZ<C>), p->np, st))) return rc;
+  if ((rc = rt::copy_d2h(hp->planes, d_planes, np * sizeof(XYZZ<C>), st))) return rc;
   if ((rc = rt::copy_d2h(hp->err, d_err, sizeof hp->err, st))) return rc;
   p->done = false;
   return PCGPU_OK;
@@ -422,9 +462,7 @@ int msm_collect(pcgpu_ctx *ctx, MsmPending<C> *p, host::HXYZZ<C> *out) {
   ctx->last_geom[PCGPU_GEOM_HEAVY] = hp->err[MSM_ERR_HEAVY];
   if (hp->err[MSM_ERR_RANGE]) return PCGPU_E_RANGE;
   auto t0 = std::chrono::steady_clock::now();
-  const host::HXYZZ<C> *planes = (const host::HXYZZ<C> *)hp->planes;
-  *out = p->g.h_split ? host::combine_bit_planes_2level<C>(planes, p->g.S, p->g.c, p->g.h_split)
-                      : host::combine_bit_planes<C>(planes, p->g.S, p->g.c);
+  *out = host::combine_bit_planes_2level<C>((const host::HXYZZ<C> *)hp->planes, p->g.S, p->g.c, p->g.h_split);
   if (ctx->prof.on) {
     ctx->prof.ms[6] += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
     ctx->prof.cnt[6]++;
@@ -488,13 +526,15 @@ int msm_peer_impl(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, cons
   for (uint32_t d = 0; d < world; d++) push.win[d] = (char *)win[d];
   push.rank = rank; push.world = world; push.epoch = epoch;
   uint32_t *d_timeout = &ctx->d_words->peer_timeout;
-  bool pipeline = n > SMALL_MAX_N || (n > 0 && !msm_small_enabled());
-  MsmGeom g;
+  MsmPlan plan;
+  if ((rc = msm_plan<C>(ctx, srs, base_offset, n, mont, &plan))) return rc;
+  bool pipeline = plan.path == PCGPU_MSM_PATH_BUCKETS;
   if (pipeline) {
-    const XYZZ<C> *d_planes = nullptr; size_t stride = 0; uint32_t *d_err = nullptr;
-    if ((rc = msm_device_planes<C>(ctx, srs, base_offset, d_scalars, n, mont, &g, &d_planes, &stride, &d_err))) return rc;
+    const XYZZ<C> *d_planes = nullptr; uint32_t *d_err = nullptr;
+    if ((rc = msm_device_planes<C>(ctx, plan, d_scalars, &d_planes, &d_err))) return rc;
+    const MsmGeom &g = plan.g;
     const size_t np = (size_t)g.S * g.c;
-    if (sizeof(PeerRecordHeader) + np * sizeof(XYZZ<C>) <= (size_t)PEER_RECORD_BYTES && stride == 1) {
+    if (sizeof(PeerRecordHeader) + np * sizeof(XYZZ<C>) <= (size_t)PEER_RECORD_BYTES) {
       push.planes = (const uint32_t *)d_planes; push.plane_words = (uint32_t)(np * sizeof(XYZZ<C>) / 4);
       push.hdr.np = (uint32_t)np; push.hdr.S = g.S; push.hdr.c = g.c; push.hdr.h_split = g.h_split; push.d_err = d_err;
     } else {
@@ -534,8 +574,7 @@ int msm_peer_impl(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, cons
     if (h.np == 0 || h.np > PCGPU_MAX_PLANES || sizeof h + (size_t)h.np * sizeof(XYZZ<C>) > (size_t)PEER_RECORD_BYTES || h.np != h.S * h.c) return PCGPU_E_PEER;
     host::HXYZZ<C> planes[PEER_RECORD_BYTES / sizeof(XYZZ<C>) + 1];
     memcpy(planes, p + sizeof h, (size_t)h.np * sizeof(XYZZ<C>));
-    acc = host::padd<C>(acc, h.h_split ? host::combine_bit_planes_2level<C>(planes, h.S, h.c, h.h_split)
-                                       : host::combine_bit_planes<C>(planes, h.S, h.c));
+    acc = host::padd<C>(acc, host::combine_bit_planes_2level<C>(planes, h.S, h.c, h.h_split));
   }
   host::to_affine<C>(acc, out_xy, out_inf);
   return PCGPU_OK;
@@ -572,17 +611,13 @@ int msm_batch_impl(pcgpu_ctx *ctx, const pcgpu_srs *srs, const void *scalars, si
     }
     return PCGPU_OK;
   }
-  CombGeom g; memset(&g, 0, sizeof g);
-  g.n_bases = (uint32_t)srs->n; g.c = srs->comb_c; g.W = (C::Fr::BITS + g.c - 1) / g.c; g.NBk = 1u << (g.c - 1);
+  CombGeom g = comb_geometry<C>(srs->n, srs->comb_c);
   g.n = (uint32_t)n; g.count = (uint32_t)count;
   g.seg_len = 64; if (count < 4096) { while (g.seg_len > 8 && count * ((n + g.seg_len - 1) / g.seg_len) < 65536) g.seg_len /= 2; }
   g.segs = (uint32_t)((n + g.seg_len - 1) / g.seg_len);
   g.scalar_bits = C::Fr::BITS; g.scalars_mont = mont ? 1 : 0;
   size_t ntasks = count * g.segs;
-  uint64_t *lg = ctx->last_geom;
-  memset(lg, 0, sizeof ctx->last_geom);
-  lg[PCGPU_GEOM_PATH] = PCGPU_MSM_PATH_COMB; lg[PCGPU_GEOM_N] = n; lg[PCGPU_GEOM_C] = g.c; lg[PCGPU_GEOM_W] = g.W;
-  lg[PCGPU_GEOM_SPLIT] = g.seg_len; lg[PCGPU_GEOM_ENTRIES] = ntasks;
+  comb_report(ctx, g);
   uint32_t *d_err; XYZZ<C> *partial; Affine<C> *d_out; const uint32_t *d_s;
   Staging io(ctx, flags);
   io.scratch(d_err, 64);
@@ -1088,7 +1123,7 @@ int ipa_round_lr_impl(pcgpu_ctx *ctx, pcgpu_ctx *sib, pcgpu_ipa *st, const void 
     const Affine<C> *key = (const Affine<C> *)st->d_key;
     MsmSmallProblem<C> pr[2] = {{key, st->d_sl, d_h, d_ip, (uint32_t)M}, {key, st->d_sr, d_h, d_ip + 8, (uint32_t)M}};
     host::HXYZZ<C> lr[2];
-    if ((rc = msm_small_to_host<C>(ctx, pr, 2, true, lr))) return rc;
+    if ((rc = msm_small_to_host<C>(ctx, msm_small_plan(M), pr, 2, true, lr))) return rc;
     host::to_affine<C>(lr[0], out_l_xy, out_l_inf);
     host::to_affine<C>(lr[1], out_r_xy, out_r_inf);
     return PCGPU_OK;
@@ -1102,7 +1137,7 @@ int ipa_round_lr_impl(pcgpu_ctx *ctx, pcgpu_ctx *sib, pcgpu_ipa *st, const void 
     MsmSmallProblem<C> pr[2] = {{key, cr, d_h, d_ip, (uint32_t)m},          // cm_commit(key_l, coeffs_r) + h' <c_r, z_l>
                                 {key + m, cl, d_h, d_ip + 8, (uint32_t)m}};  // cm_commit(key_r, coeffs_l) + h' <c_l, z_r>
     host::HXYZZ<C> lr[2];
-    if ((rc = msm_small_to_host<C>(ctx, pr, 2, true, lr))) return rc;
+    if ((rc = msm_small_to_host<C>(ctx, msm_small_plan(m), pr, 2, true, lr))) return rc;
     host::to_affine<C>(lr[0], out_l_xy, out_l_inf);
     host::to_affine<C>(lr[1], out_r_xy, out_r_inf);
     return PCGPU_OK;
@@ -1187,7 +1222,7 @@ int ipa_finish_impl(pcgpu_ctx *ctx, pcgpu_ipa *st, void *out_final_key_xy, void 
   if (out_final_key_xy && st->frozen_m) {   // final_comm_key = sum_j w[j] B[j]
     MsmSmallProblem<C> pr{(const Affine<C> *)st->d_key, st->d_w, nullptr, nullptr, (uint32_t)st->frozen_m};
     host::HXYZZ<C> k;
-    if ((rc = msm_small_to_host<C>(ctx, &pr, 1, true, &k))) return rc;
+    if ((rc = msm_small_to_host<C>(ctx, msm_small_plan(st->frozen_m), &pr, 1, true, &k))) return rc;
     uint8_t inf = 0;
     host::to_affine<C>(k, out_final_key_xy, &inf);
   } else if (out_final_key_xy && (rc = rt::copy_d2h(out_final_key_xy, st->d_key, sizeof(Affine<C>), s))) return rc;
@@ -1870,8 +1905,7 @@ inline int measure_imad_peak_impl(pcgpu_ctx *ctx, double *ops_per_s) {
 // (inst_unit.cu is built once per (curve, group); `EXT` = extern declares, empty defines).  The three msm_* helpers are
 // instantiated in ONE group and only declared elsewhere, so the Pippenger kernels are compiled exactly once per curve.
 #define PCGPU_INST_PIPE(C, EXT)                                                                                            \
-  EXT template int msm_device_planes<C>(pcgpu_ctx *, const pcgpu_srs *, size_t, const uint32_t *, size_t, bool, MsmGeom *, \
-                                        const XYZZ<C> **, size_t *, uint32_t **);                                          \
+  EXT template int msm_device_planes<C>(pcgpu_ctx *, const MsmPlan &, const uint32_t *, const XYZZ<C> **, uint32_t **);  \
   EXT template int msm_to_host<C>(pcgpu_ctx *, const pcgpu_srs *, size_t, const uint32_t *, size_t, bool, host::HXYZZ<C> *); \
   EXT template int msm_issue<C>(pcgpu_ctx *, const pcgpu_srs *, size_t, const uint32_t *, size_t, bool, MsmPending<C> *);   \
   EXT template int msm_collect<C>(pcgpu_ctx *, MsmPending<C> *, host::HXYZZ<C> *);
@@ -1886,7 +1920,7 @@ inline int measure_imad_peak_impl(pcgpu_ctx *ctx, double *ops_per_s) {
   EXT template int pcgpu::msm_reduce_launch<C>(const MsmGeom &, const uint32_t *, const XYZZ<C> *, XYZZ<C> *, XYZZ<C> *, XYZZ<C> *,    \
                                         const uint32_t *, const uint32_t *, rt::stream_t);
 #define PCGPU_INST_SMALL(C, EXT)                                                                                           \
-  EXT template int msm_small_to_host<C>(pcgpu_ctx *, const MsmSmallProblem<C> *, uint32_t, bool, host::HXYZZ<C> *);
+  EXT template int msm_small_to_host<C>(pcgpu_ctx *, const MsmPlan &, const MsmSmallProblem<C> *, uint32_t, bool, host::HXYZZ<C> *);
 #define PCGPU_INST_SRS(C, EXT)                                                                                             \
   EXT template int srs_register_impl<C>(pcgpu_ctx *, const void *, const uint8_t *, size_t, uint32_t, pcgpu_srs *);        \
   EXT template int msm_impl<C>(pcgpu_ctx *, const pcgpu_srs *, size_t, const void *, size_t, uint32_t, void *, uint8_t *, void *); \

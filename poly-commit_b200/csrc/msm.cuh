@@ -47,7 +47,7 @@ struct MsmGeom {
                           // 2^h * sum_hi hi * R_hi + sum_lo (lo+1) * C_lo over row sums R and column sums C (large c)
   uint32_t pt_words;      // table record stride in 32-bit words (2N raw; 32 for 128-byte aligned BLS12-381 records)
   uint32_t y_words;       // offset of y inside a record, in words (N raw; 16 in the aligned BLS12-381 layout)
-  uint32_t pair_tdiv;     // the pair-round kernel runs with 1 / pair_tdiv of a full wave of threads (see msm_run)
+  uint32_t pair_tdiv;     // the pair-round kernel runs with 1 / pair_tdiv of a full wave of threads (msm_plan; 0 without rounds)
 };
 
 enum : uint32_t { ENTRY_SIGN = 0x80000000u, ENTRY_GROUP_SHIFT = 26, ENTRY_IDX_MASK = (1u << 26) - 1 };
@@ -544,26 +544,33 @@ inline uint32_t msm_pick_c(size_t n) {
 }
 
 inline MsmGeom msm_geometry(size_t n, uint32_t c, uint32_t groups, uint32_t scalar_bits, bool mont,
-                            uint64_t table_stride, uint64_t base_off) {
-  MsmGeom g;
+                            uint64_t table_stride, uint64_t base_off, uint32_t L) {
+  MsmGeom g{};   // affine_rounds, pair_tdiv: set by msm_plan; pt_words, y_words: by the caller (table_layout)
   g.n = (uint32_t)n; g.c = c;
   g.W = (scalar_bits + c - 1) / c;   // enough because load_scalar halves the scalar range (see there)
   g.G = groups < 1 ? 1 : groups;
   g.S = (g.W + g.G - 1) / g.G;
   g.NB = 1u << (c - 1);
   g.TB = g.S * g.NB;
-  g.L = 32;
-  if (const char *e = getenv("PCGPU_MSM_L")) { int v = atoi(e); if (v >= 4 && v <= 4096) g.L = (uint32_t)v; }  // tuning knob
+  g.L = L;
   g.seg_len = 16;
   g.nseg = (g.NB + g.seg_len - 1) / g.seg_len;
   g.scalar_bits = scalar_bits; g.scalars_mont = mont ? 1 : 0;
   g.table_stride = table_stride; g.base_off = base_off;
-  g.affine_rounds = 0;
   g.h_split = (c - 1) / 2;
-  g.pt_words = 0; g.y_words = 0;  // set by the caller (table_layout)
-  g.pair_tdiv = 1;
   return g;
 }
+
+// One MSM as decided before its first launch (impl.cuh msm_plan): the path and, for the bucket pipeline, all msm_run needs.
+struct MsmPlan {
+  uint32_t path;           // PCGPU_MSM_PATH_NONE / _SMALL / _BUCKETS (include/pcgpu.h)
+  uint64_t n;              // terms (small path: of the longest problem)
+  uint32_t split;          // small path: blocks per window
+  MsmGeom g;               // bucket path: the kernels' geometry, affine_rounds and pair_tdiv included
+  const uint32_t *tables;  // bucket path: the raw bases or the window-folded records
+  size_t wave;             // threads of one resident wave of the pair kernel, against which R was chosen (0 on G2)
+  uint32_t T;              // pair-round threads (0 without pair rounds)
+};
 
 // XYZZ scratch elements of the reduction stage: row sums and column sums of every set
 inline size_t msm_plane_scratch_elems(const MsmGeom &g) {
@@ -616,18 +623,17 @@ int msm_reduce_launch(const MsmGeom &g, const uint32_t *task_off, const XYZZ<C> 
   return rt::launch_blocks<REDUCE_BLOCK>(MsmPlaneReduceBody<C>{Rv, Cv, plane_out, rows, cols, bits_c, bits_r}, (size_t)g.S * (bits_c + bits_r), smem, st);
 }
 
-// Runs the device pipeline on `st`.  d_scalars: n x 8 uint32 on the device.  On return (asynchronously)
-// *d_planes points at the S*c bit-plane sums, element (s*c + j) at index (s*c + j) * plane_stride, and
-// *d_err at the run's MSM_ERR_WORDS error words.  `prof` brackets stages with events.
-// *pair_threads / *pair_tdiv (if given) receive the pair-round kernel's thread count and wave divisor (0 without rounds).
+// Runs the bucket pipeline of `plan` on `st`.  d_scalars: n x 8 uint32 on the device.  On return (asynchronously) *d_planes
+// points at the S*c bit-plane sums, packed, and *d_err at the run's MSM_ERR_WORDS error words.  `prof` brackets stages with
+// events.  pow2: the fp_inv_gcd table of the pair rounds (needed when plan.g.affine_rounds > 0).
 template <class C, class Prof>
-inline int msm_run(const uint32_t *tables, const MsmGeom &g, const uint32_t *d_scalars, rt::Arena &arena,
-                   const XYZZ<C> **d_planes, size_t *plane_stride, uint32_t **d_err_out, rt::stream_t st, Prof &prof,
-                   const uint32_t *pow2 = nullptr, uint32_t *pair_threads = nullptr, uint32_t *pair_tdiv = nullptr) {
+inline int msm_run(const MsmPlan &plan, const uint32_t *d_scalars, rt::Arena &arena, const XYZZ<C> **d_planes,
+                   uint32_t **d_err_out, rt::stream_t st, Prof &prof, const uint32_t *pow2) {
   using QF = Fp<typename C::Fq>;
+  const MsmGeom &g = plan.g;
   const size_t max_entries = (size_t)g.n * g.W, max_tasks = max_entries / g.L + g.TB + 1;
   const size_t bound0 = max_entries / 2 + g.TB + 1, bound1 = bound0 / 2 + g.TB + 1;   // pair-round output bounds
-  const bool pair_rounds = C::EXT == 1 && g.affine_rounds && pow2;   // G2 (C::EXT == 2) runs with R = 0: no pair-round kernels
+  const bool pair_rounds = C::EXT == 1 && g.affine_rounds;   // G2 (C::EXT == 2) runs with R = 0: no pair-round kernels
   uint32_t *counts, *offsets, *cursor, *ntasks, *task_off, *task_bucket, *entries, *scratch, *err;
   XYZZ<C> *partial, *buckets, *planes, *plane_out;
   uint32_t *offA = nullptr, *offB = nullptr, *cnt = nullptr, *src = nullptr;
@@ -644,7 +650,7 @@ inline int msm_run(const uint32_t *tables, const MsmGeom &g, const uint32_t *d_s
     }
   });
   if (rc) return rc;
-  *d_err_out = err; *d_planes = plane_out; *plane_stride = 1;
+  *d_err_out = err; *d_planes = plane_out;
 
   prof.begin(0, st);
   if ((rc = rt::dev_memset(counts, 0, (g.TB + 2) * sizeof(uint32_t), st))) return rc;
@@ -664,18 +670,6 @@ inline int msm_run(const uint32_t *tables, const MsmGeom &g, const uint32_t *d_s
   // ---- batched-affine pairwise rounds (msm_affine.cuh): halve every bucket g.affine_rounds times ----
   const Affine<C> *pts = nullptr;
   if constexpr (C::EXT == 1) if (pair_rounds) {
-    size_t Tmax = 0;
-    if ((rc = msm_pair_oneshot_threads<C>(&Tmax))) return rc;
-    if (Tmax > (1u << 20)) Tmax = 1u << 20;
-    // Throughput mode (several MSM pipelines in flight on sibling streams): half a wave per pair kernel, so that the pair kernels
-    // of TWO pipelines are co-resident on every SM -- a full wave owns the whole register file -- and the DRAM-bound pass 1 and
-    // the ALU-bound inversion of one overlap the multiply-bound pass 2 of the other; every thread then covers twice the slots
-    // with the same single inversion per round.
-    uint32_t tdiv = g.pair_tdiv ? g.pair_tdiv : 1;
-    if (const char *e = getenv("PCGPU_MSM_AFFINE_TDIV")) { int v = atoi(e); if (v >= 1 && v <= 16) tdiv = (uint32_t)v; }  // tuning knob
-    if (tdiv > 1) Tmax = (Tmax / tdiv + 127) / 128 * 128;
-    if (pair_threads) *pair_threads = (uint32_t)Tmax;
-    if (pair_tdiv) *pair_tdiv = tdiv;
     prof.begin(11, st);
     const uint32_t *off_in = offsets;
     size_t bound = max_entries;
@@ -687,9 +681,8 @@ inline int msm_run(const uint32_t *tables, const MsmGeom &g, const uint32_t *d_s
       if ((rc = rt::launch<256>(PairCountBody{off_in, cnt}, g.TB, st))) return rc;
       if ((rc = exclusive_scan_u32(cnt, g.TB, off_out, scratch, st))) return rc;
       if ((rc = rt::launch<256>(PairPlanBody{off_in, off_out, g.TB, src}, bound, st))) return rc;
-      uint32_t T = (uint32_t)Tmax;
       if (r == 0) prof.begin(12, st);
-      rc = msm_pair_round_oneshot<C>(r == 0, tables, g, entries, in, src, off_out, T, (uint32_t *)prefix, pow2, out, st);
+      rc = msm_pair_round_oneshot<C>(r == 0, plan.tables, g, entries, in, src, off_out, plan.T, (uint32_t *)prefix, pow2, out, st);
       if (rc) return rc;
       if (r == 0) prof.end(12, st);
       off_in = off_out;
@@ -707,7 +700,7 @@ inline int msm_run(const uint32_t *tables, const MsmGeom &g, const uint32_t *d_s
   prof.end(3, st);
 
   prof.begin(4, st);
-  if ((rc = msm_accumulate_launch<C>(tables, g, offsets, task_off, task_bucket, entries, partial, err + MSM_ERR_QUEUE, pts, st))) return rc;
+  if ((rc = msm_accumulate_launch<C>(plan.tables, g, offsets, task_off, task_bucket, entries, partial, err + MSM_ERR_QUEUE, pts, st))) return rc;
   prof.end(4, st);
 
   prof.begin(5, st);

@@ -44,10 +44,6 @@ inline int dev_memset(void *p, int v, size_t bytes, stream_t) { memset(p, v, byt
 inline int copy_h2d(void *d, const void *h, size_t bytes, stream_t) { memcpy(d, h, bytes); return OK; }
 inline int copy_d2h(void *h, const void *d, size_t bytes, stream_t) { memcpy(h, d, bytes); return OK; }
 inline int copy_d2d(void *d, const void *s, size_t bytes, stream_t) { memmove(d, s, bytes); return OK; }
-inline int copy_d2h_2d(void *h, size_t hpitch, const void *d, size_t dpitch, size_t width, size_t rows, stream_t) {
-  for (size_t r = 0; r < rows; r++) memcpy((char *)h + r * hpitch, (const char *)d + r * dpitch, width);
-  return OK;
-}
 inline int stream_sync(stream_t) { return OK; }
 inline int last_error() { return OK; }
 typedef int event_t;
@@ -71,7 +67,6 @@ inline uint32_t next_task(uint32_t *counter) { return atomic_add(counter, 1u); }
 template <int BLOCK, class Body>
 inline int launch_persistent(const Body &body, stream_t) { body(0); return OK; }
 // threads of one resident wave of `Body` (host emulation: a small number so multi-iteration paths are exercised)
-template <int BLOCK, class Body> inline int resident_threads(size_t *out) { *out = 48; return OK; }
 template <int BLOCK, int MINB, class Body> inline int launch_occ(const Body &body, size_t n, stream_t s) { return launch<BLOCK>(body, n, s); }
 template <int BLOCK, int MINB, class Body> inline int resident_threads_occ(size_t *out) { *out = 48; return OK; }
 // Block-cooperative bodies: body(block_id, shared_memory).  Work inside the body is written as
@@ -107,9 +102,6 @@ inline int dev_memset(void *p, int v, size_t bytes, stream_t s) { return map_cud
 inline int copy_h2d(void *d, const void *h, size_t bytes, stream_t s) { return map_cuda(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, s)); }
 inline int copy_d2h(void *h, const void *d, size_t bytes, stream_t s) { return map_cuda(cudaMemcpyAsync(h, d, bytes, cudaMemcpyDeviceToHost, s)); }
 inline int copy_d2d(void *d, const void *s_, size_t bytes, stream_t s) { return map_cuda(cudaMemcpyAsync(d, s_, bytes, cudaMemcpyDeviceToDevice, s)); }
-inline int copy_d2h_2d(void *h, size_t hpitch, const void *d, size_t dpitch, size_t width, size_t rows, stream_t s) {
-  return map_cuda(cudaMemcpy2DAsync(h, hpitch, d, dpitch, width, rows, cudaMemcpyDeviceToHost, s));
-}
 inline int stream_sync(stream_t s) { return map_cuda(cudaStreamSynchronize(s)); }
 inline int last_error() { return map_cuda(cudaGetLastError()); }
 typedef cudaEvent_t event_t;
@@ -209,20 +201,6 @@ __device__ __forceinline__ uint32_t next_task(uint32_t *counter) {
 template <class Body, int BLOCK>
 __global__ void __launch_bounds__(BLOCK) run_persistent_kernel(const Body body) {
   body((size_t)blockIdx.x * BLOCK + threadIdx.x);
-}
-template <int BLOCK, class Body>
-inline int resident_threads(size_t *out) {
-  static size_t cached = 0;
-  if (!cached) {
-    int dev = 0, sms = 0, per_sm = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, run_kernel<Body, BLOCK>, BLOCK, 0);
-    if (e != cudaSuccess) return map_cuda(e);
-    cached = (size_t)sms * (per_sm > 0 ? per_sm : 1) * BLOCK;
-  }
-  *out = cached;
-  return OK;
 }
 template <int BLOCK, class Body>
 inline int launch_persistent(const Body &body, stream_t s) {

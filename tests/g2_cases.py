@@ -10,10 +10,10 @@ import os
 import numpy as np
 
 from oracle import pyref
-from tests import util
+from tests import msm_cases, util
 
 PAIRING = ["bls12_381", "bn254"]
-SMALL_MAX_N = 4096
+SMALL_MAX_N = msm_cases.SMALL_MAX_N
 _KATS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "external_kats.json")
 
 
@@ -85,25 +85,6 @@ def fr_limbs(vals, mont=False, cname=None):
     return a
 
 
-def msm_pick_c(n):
-    return min(16, max(8, max(n, 1).bit_length() - 1 - 4))
-
-
-def check_geometry(eng, pc, cname, n, path):
-    """the G2 MSM of n terms took `path` ("small" or "buckets"); the bucket pipeline runs on raw bases without pair rounds"""
-    g = eng.msm_last_geometry()
-    if n == 0:
-        assert g["path"] == pc.binding.MSM_PATH_NONE, g
-        return
-    if path == "small" and n <= SMALL_MAX_N:
-        assert g["path"] == pc.binding.MSM_PATH_SMALL and g["n"] == n, g
-        return
-    c = int(os.environ.get("PCGPU_MSM_C") or msm_pick_c(n))
-    W = -(-pyref.Curve(cname).r.bit_length() // c)
-    assert g["path"] == pc.binding.MSM_PATH_BUCKETS and (g["n"], g["c"], g["W"], g["G"]) == (n, c, W, 1), g
-    assert (g["R"], g["T"], g["entries"]) == (0, 0, n * W), g
-
-
 def msm(eng, pc, cname, bases, scalars, inf=None, mont=False):
     """one G2 MSM through a registered key -> affine point or None"""
     srs = eng.srs_register(group(pc, cname), bases, inf=inf)
@@ -166,7 +147,7 @@ def generator_kat_case(eng, pc, cname, path):
     assert G.on_curve(H)
     hx, _ = to_limbs(cname, [H, H])
     assert msm(eng, pc, cname, hx, fr_limbs([G.r - 1, 1])) is None
-    check_geometry(eng, pc, cname, 2, path)
+    msm_cases.check_geometry(eng, pc, cname, 2, g2=True, small=path == "small")
     assert msm(eng, pc, cname, hx[:1], fr_limbs([2])) == G.add(H, H)
     xy, is_inf = eng.msm_bases(group(pc, cname), hx, fr_limbs([3, 2]))     # unregistered bases
     assert from_limbs(cname, xy, is_inf) == G.mul(5, H)
@@ -177,7 +158,7 @@ def edge_case(eng, pc, cname, path, seed=1):
     an exact zero sum; canonical and Montgomery scalars; PCGPU_E_RANGE followed by a correct MSM on the same context"""
     G = pyref.G2(cname)
     r = G.r
-    c = msm_pick_c(1) if path == "small" else int(os.environ.get("PCGPU_MSM_C") or msm_pick_c(64))
+    c = msm_cases.msm_pick_c(1) if path == "small" else int(os.environ.get("PCGPU_MSM_C") or msm_cases.msm_pick_c(64))
     half = 1 << (c - 1)
     alt = sum(half << (c * w) for w in range(256 // c)) % r          # every window +2^(c-1) (a carry chain of -2^(c-1) digits)
     ks = [int(v) for v in util.rand_fr_ints(cname, 24, seed)]
@@ -195,13 +176,13 @@ def edge_case(eng, pc, cname, path, seed=1):
             sc = fr_limbs(ss[:n], mont, cname)
             got = msm(eng, pc, cname, bases[:n], sc, inf=inf[:n], mont=mont)
             assert got == trapdoor_expect(cname, ks[:n], ss[:n]), (cname, path, mont, n)
-            check_geometry(eng, pc, cname, n, path)
+            msm_cases.check_geometry(eng, pc, cname, n, g2=True, small=path == "small")
     # an exact zero sum: every term cancels against a negated copy
     kz = ks[:8] + [(r - k) % r for k in ks[:8]]
     bz = trapdoor_bases(eng, pc, cname, kz, sample=2, seed=seed)
     sz = ss[:8] * 2
     assert msm(eng, pc, cname, bz, fr_limbs(sz)) is None
-    check_geometry(eng, pc, cname, 16, path)
+    msm_cases.check_geometry(eng, pc, cname, 16, g2=True, small=path == "small")
     # out-of-range scalars, then a good MSM on the same context
     srs = eng.srs_register(group(pc, cname), bases)
     for bad in (r, (1 << 256) - 1):
@@ -227,7 +208,7 @@ def random_vs_pyref_case(eng, pc, cname, n, path, seed=2):
     for P, s in zip(pts, ss):
         exp = G.add(exp, G.mul(s, P))
     assert msm(eng, pc, cname, bases, fr_limbs(ss)) == exp, (cname, n)
-    check_geometry(eng, pc, cname, n, path)
+    msm_cases.check_geometry(eng, pc, cname, n, g2=True, small=path == "small")
 
 
 def fr_ints(arr):
@@ -254,7 +235,7 @@ def trapdoor_case(eng, pc, cname, n, path, skewed=False, seed=3, sample=16, keye
         ss = fr_ints(util.rand_fr(cname, n, seed + 1, mont=False))
     mont = bool(seed & 1)
     assert msm(eng, pc, cname, bases, fr_limbs(ss, mont, cname), mont=mont) == trapdoor_expect(cname, ks, ss), (cname, n, skewed)
-    check_geometry(eng, pc, cname, n, path)
+    msm_cases.check_geometry(eng, pc, cname, n, g2=True, small=path == "small")
 
 
 def g2_id_rejected_case(eng, pc, cname):

@@ -3,14 +3,18 @@ sizes where the pair rounds run at depth on an H100), plus the restatement of th
 asserts through Engine.msm_last_geometry: a case whose geometry differs from the one it claims to cover fails, so coverage
 cannot silently move to another path when the picker or the pair kernel's occupancy changes.
 
-The policy restated here (csrc/msm.cuh msm_pick_c / msm_geometry, csrc/srs.cuh srs_precompute_window, csrc/impl.cuh
-msm_device_planes, msm_run):
+The policy restated here is the one csrc/impl.cuh msm_plan decides (with csrc/msm.cuh msm_pick_c / msm_geometry and
+csrc/srs.cuh srs_precompute_window); it is the suite's only copy, G2 cases (tests/g2_cases.py) included:
+  * n = 0: no MSM (path NONE, every word 0);
+  * n <= SMALL_MAX_N with PCGPU_MSM_SMALL unset or not "0": the one-launch kernel, split = 1 block per window below 512 terms,
+    else 3;
   * window-folded tables (SRS_PRECOMPUTE, n >= 4096): c = the registration's window, G = W table groups, one bucket set;
   * raw bases: c = clamp(floor(log2 n) - 4, 8, 16) or PCGPU_MSM_C, G = 1, S = W bucket sets;
   * W = ceil(bits(r) / c); entries = n * W; buckets TB = S * 2^(c-1);
   * affine rounds R: add one while R < 8, (entries / TB) >> R >= 4 and entries >> (R + 1) >= 16 * wave, where wave is one
-    resident wave of the pair kernel; PCGPU_MSM_AFFINE_ROUNDS overrides;
-  * pair threads T = wave, or with a divisor tdiv > 1 (batch mode, PCGPU_MSM_AFFINE_TDIV) ceil(wave / tdiv / 128) * 128.
+    resident wave of the pair kernel; PCGPU_MSM_AFFINE_ROUNDS overrides; G2: R = 0 and wave = 0;
+  * pair threads T = wave, or with a divisor tdiv > 1 (batch mode, PCGPU_MSM_AFFINE_TDIV) ceil(wave / tdiv / 128) * 128;
+    T = tdiv = 0 without rounds.
 """
 import os
 
@@ -20,6 +24,9 @@ from oracle import orc, pyref
 from tests import util
 
 SRS_PRECOMPUTE_MIN_N = 1 << 12
+SMALL_MAX_N = 4096              # csrc/msm_small.cuh: the one-launch kernel's largest problem
+SMALL_SPLIT_MIN_N = 512         # csrc/msm_small.cuh: from this many terms a window is split over SMALL_SPLIT blocks
+SMALL_SPLIT = 3
 HEAVY_BUCKET_TASKS = 8          # csrc/msm.cuh: a bucket with more accumulate tasks than this goes to MsmHeavyBucketBody
 HEAVY_GRID = 64                 # blocks of MsmHeavyBucketBody (grid-strided over the heavy list)
 DEPTH_SLOTS = 32                # a "depth" case gives every pair-round thread at least this many round-0 slots
@@ -51,13 +58,22 @@ def pair_threads(wave, tdiv):
     return t if tdiv == 1 else (t // tdiv + 127) // 128 * 128
 
 
-def check_geometry(eng, pc, cname, n, folded_c=None, tdiv=1, depth=False):
-    """asserts that the last MSM on `eng` took the bucket pipeline with the documented geometry for n terms.  folded_c: the
-    window the SRS_PRECOMPUTE tables were registered with (None: raw bases).  tdiv: the pair-round divisor expected without
-    a PCGPU_MSM_AFFINE_TDIV knob.  depth: the pair rounds must run and give every thread >= DEPTH_SLOTS round-0 slots."""
+def check_geometry(eng, pc, cname, n, folded_c=None, tdiv=1, depth=False, g2=False, small=False):
+    """asserts every word of the report of the last MSM on `eng`, an MSM of n terms.  n = 0 took no path; with small (the
+    one-launch kernel enabled) n <= SMALL_MAX_N took it; every other MSM took the bucket pipeline with the documented
+    geometry.  folded_c: the window the SRS_PRECOMPUTE tables were registered with (None: raw bases).  tdiv: the pair-round
+    divisor expected without a PCGPU_MSM_AFFINE_TDIV knob.  depth: the pair rounds must run and give every thread
+    >= DEPTH_SLOTS round-0 slots.  g2: a G2 MSM (raw bases, no pair rounds).  Returns the report."""
     g = eng.msm_last_geometry()
+    if n == 0:
+        assert g == dict.fromkeys(g, 0), g
+        return g
+    if small and n <= SMALL_MAX_N:
+        split = SMALL_SPLIT if n >= SMALL_SPLIT_MIN_N else 1
+        assert g == dict(dict.fromkeys(g, 0), path=pc.binding.MSM_PATH_SMALL, n=n, split=split), g
+        return g
     bits = pyref.Curve(cname).r.bit_length()
-    assert g["path"] == pc.binding.MSM_PATH_BUCKETS and g["n"] == n, g
+    assert g["path"] == pc.binding.MSM_PATH_BUCKETS and g["n"] == n and g["split"] == 0, g
     if folded_c is not None and n >= SRS_PRECOMPUTE_MIN_N:
         c = folded_c
         G = -(-bits // c)
@@ -69,14 +85,20 @@ def check_geometry(eng, pc, cname, n, folded_c=None, tdiv=1, depth=False):
     entries = n * W
     assert g["entries"] == entries, g
     S = -(-W // G)
-    knob = os.environ.get("PCGPU_MSM_AFFINE_ROUNDS")
-    R = int(knob) if knob else policy_rounds(entries, S << (c - 1), g["wave"])
+    if g2:
+        assert g["wave"] == 0, g
+        R = 0
+    else:
+        assert g["wave"] > 0, g
+        knob = os.environ.get("PCGPU_MSM_AFFINE_ROUNDS")
+        R = int(knob) if knob else policy_rounds(entries, S << (c - 1), g["wave"])
     assert g["R"] == R, (g, R)
     if R:
         td = int(os.environ.get("PCGPU_MSM_AFFINE_TDIV") or tdiv)
         assert (g["T"], g["tdiv"]) == (pair_threads(g["wave"], td), td), g
     else:
-        assert g["T"] == 0, g
+        assert (g["T"], g["tdiv"]) == (0, 0), g
+    assert g["heavy"] is not None, g
     if depth:
         assert R >= 1 and entries // (2 * g["T"]) >= DEPTH_SLOTS, g
     return g
