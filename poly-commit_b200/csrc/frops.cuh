@@ -140,62 +140,6 @@ struct DivChunkWriteBody {
   }
 };
 
-// Chunk carries in ONE launch (replaces the fold / carry levels above for up to DIV_SCAN_BLOCK * 4096 chunks): the chunk values
-// obey  out_c = local_c + z^K * out_{c+1}  (out beyond the top chunk = 0), a reverse linear recurrence.  One block: thread t walks
-// its segment of S consecutive chunks (Horner, top down), the DIV_SCAN_BLOCK segment values are combined by a reverse
-// Hillis-Steele scan in shared memory (E_t += W^(2^k) E_(t + 2^k), W = z^(K S)), and every thread replays its segment writing
-// the value that ENTERS each chunk (`carry`), which DivChunkWriteBody consumes.  The value leaving chunk 0 is the remainder p(z).
-enum { DIV_SCAN_BLOCK = 1024 };
-template <class R>
-struct DivBlockScanBody {
-  const uint32_t *local; size_t nchunks; const uint32_t *z; uint32_t *carry; uint32_t *rem;
-  PCGPU_KERNEL_DEV void operator()(size_t, uint32_t *smem) const {
-    const size_t S = (nchunks + DIV_SCAN_BLOCK - 1) / DIV_SCAN_BLOCK;     // chunks per thread
-    uint32_t *bufA = smem, *bufB = smem + 8 * DIV_SCAN_BLOCK, *pw = smem + 16 * DIV_SCAN_BLOCK;   // pw[0] = z^K, pw[1] = W^(2^k)
-    PCGPU_BLOCK_FOR(t, 1) {
-      Fp<R> a = load_fr<R>(z, 0);
-      for (int k = DIV_K; k > 1; k >>= 1) a = fp_sqr<R>(a);
-      store_fr<R>(pw, 0, a);                                              // z^K
-      Fp<R> w = Fp<R>::one(), b = a;                                      // W = (z^K)^S by square-and-multiply
-      for (size_t e = S; e; e >>= 1) { if (e & 1) w = fp_mul<R>(w, b); b = fp_sqr<R>(b); }
-      store_fr<R>(pw, 1, w);
-    }
-    PCGPU_BLOCK_SYNC();
-    PCGPU_BLOCK_FOR(t, DIV_SCAN_BLOCK) {
-      const size_t lo = (size_t)t * S, hi = lo + S < nchunks ? lo + S : nchunks;
-      const Fp<R> zk = load_fr<R>(pw, 0);
-      Fp<R> acc = Fp<R>::zero();
-      for (size_t c = hi; c-- > lo;) acc = fp_add<R>(fp_mul<R>(acc, zk), load_fr<R>(local, c));
-      store_fr<R>(bufA, t, acc);
-    }
-    PCGPU_BLOCK_SYNC();
-    uint32_t *x = bufA, *y = bufB;
-    for (uint32_t d = 1; d < DIV_SCAN_BLOCK; d <<= 1) {
-      PCGPU_BLOCK_FOR(t, DIV_SCAN_BLOCK) {
-        Fp<R> v = load_fr<R>(x, t);
-        if (t + d < DIV_SCAN_BLOCK) v = fp_add<R>(v, fp_mul<R>(load_fr<R>(pw, 1), load_fr<R>(x, t + d)));
-        store_fr<R>(y, t, v);
-      }
-      PCGPU_BLOCK_SYNC();
-      PCGPU_BLOCK_FOR(t, 1) { store_fr<R>(pw, 1, fp_sqr<R>(load_fr<R>(pw, 1))); }
-      PCGPU_BLOCK_SYNC();
-      uint32_t *tmp = x; x = y; y = tmp;
-    }
-    // x[t] = value leaving segment t's lowest chunk; the value entering segment t from above is x[t + 1]
-    PCGPU_BLOCK_FOR(t, DIV_SCAN_BLOCK) {
-      const size_t lo = (size_t)t * S, hi = lo + S < nchunks ? lo + S : nchunks;
-      const Fp<R> zk = load_fr<R>(pw, 0);
-      Fp<R> in = t + 1 < DIV_SCAN_BLOCK ? load_fr<R>(x, t + 1) : Fp<R>::zero();
-      for (size_t c = hi; c-- > lo;) {
-        store_fr<R>(carry, c, in);
-        in = fp_add<R>(fp_mul<R>(in, zk), load_fr<R>(local, c));
-      }
-      if (t == 0 && rem) store_fr<R>(rem, 0, in);
-    }
-  }
-};
-
-
 // ---------------------------------------------------------------------------------------------
 // Division by (X - z) in ONE pass over the coefficients: tiles of DIVT_TILE coefficients staged through shared memory
 // (coalesced 16-byte granules in and out, padded so that a thread's private run of DIVT_L elements is bank-conflict free),
@@ -402,64 +346,80 @@ struct DivTileBody {
   }
 };
 
-inline size_t div_scratch_words(size_t n) {
-  size_t cnt = (n + DIV_K - 1) / DIV_K, tot = 0;
-  for (int l = 0; l < DIV_MAX_LEVELS; l++) { tot += 2 * cnt; if (cnt <= DIV_F) break; cnt = (cnt + DIV_F - 1) / DIV_F; }
-  const size_t ntiles = (n + DIVT_TILE - 1) / DIVT_TILE;
-  return 8 * (tot + DIV_MAX_LEVELS + 4 + DIVT_POW_COUNT + 2 * ntiles + 4) + ntiles + 72;
+// How one division by (X - z) of n coefficients runs, decided before its first launch: the path and the layout of its scratch
+// (offsets in 32-bit words from the start of the scratch).
+//   tiles: powers (DIVT_POW_COUNT elements) at 0 | tile aggregates | tile inclusive values | control words (2 + ntiles)
+//   tree:  level factors (DIV_MAX_LEVELS elements) at 0 | per level: the nodes' local values, then their carries
+enum { DIV_PATH_NONE, DIV_PATH_TILES, DIV_PATH_TREE };
+struct DivPlan {
+  size_t n;
+  int path;                   // DIV_PATH_NONE for n = 0 (no kernel: the remainder is zero)
+  uint32_t ntiles;            // tiles
+  size_t agg, inc, ctl;       // tiles
+  int levels;                 // tree
+  size_t cnt[DIV_MAX_LEVELS], local[DIV_MAX_LEVELS], carry[DIV_MAX_LEVELS];   // tree: nodes and offsets per level
+  size_t words;               // the scratch the division needs
+};
+
+// One pass up to 2^21 coefficients; beyond that the level tree's fewer products per coefficient win.
+// PCGPU_DIV_MODE = tile | tree forces one.
+inline DivPlan div_plan(size_t n) {
+  DivPlan d{};
+  d.n = n;
+  bool tiles = n <= ((size_t)1 << 21);
+  if (const char *e = getenv("PCGPU_DIV_MODE")) tiles = e[0] == 't' && e[1] == 'i';
+  if (n == 0) {
+    d.path = DIV_PATH_NONE;
+  } else if (tiles) {
+    d.path = DIV_PATH_TILES;
+    d.ntiles = (uint32_t)((n + DIVT_TILE - 1) / DIVT_TILE);
+    d.agg = 8 * DIVT_POW_COUNT; d.inc = d.agg + 8 * (size_t)d.ntiles; d.ctl = d.inc + 8 * (size_t)d.ntiles;
+    d.words = d.ctl + 2 + d.ntiles;
+  } else {
+    d.path = DIV_PATH_TREE;
+    size_t cur = 8 * DIV_MAX_LEVELS;
+    for (size_t c = (n + DIV_K - 1) / DIV_K;; c = (c + DIV_F - 1) / DIV_F) {
+      d.cnt[d.levels] = c; d.local[d.levels] = cur; cur += 8 * c; d.carry[d.levels] = cur; cur += 8 * c;
+      d.levels++;
+      if (c <= DIV_F || d.levels == DIV_MAX_LEVELS) break;
+    }
+    d.words = cur;
+  }
+  return d;
 }
 
-// which division runs for n coefficients (see fr_div_linear)
-inline bool div_one_pass(size_t n) {
-  bool one_pass = n <= ((size_t)1 << 21);
-  if (const char *e = getenv("PCGPU_DIV_MODE")) one_pass = e[0] == 't' && e[1] == 'i';
-  return one_pass;
-}
 // The one-pass kernel's look-back is a BOUNDED spin: a tile that never sees its predecessor publish (which would take a lost
 // block, i.e. a device fault) gives up, raises ctl[1] and lets the kernel finish -- never a hang.  Callers read the word back
-// here once the stream is idle and turn it into an error code instead of returning a wrong quotient.
-inline int fr_div_check(const uint32_t *scratch, size_t n, rt::stream_t st) {
-  if (n == 0 || !div_one_pass(n)) return rt::OK;
-  const size_t ntiles = (n + DIVT_TILE - 1) / DIVT_TILE;
-  const uint32_t *ctl = scratch + 8 * DIVT_POW_COUNT + 16 * ntiles;
+// here, with the plan the division ran, once the stream is idle and turn it into an error code instead of returning a wrong
+// quotient.
+inline int fr_div_check(const DivPlan &d, const uint32_t *scratch, rt::stream_t st) {
+  if (d.path != DIV_PATH_TILES) return rt::OK;
   uint32_t h = 0;
-  int rc = rt::copy_d2h(&h, ctl + 1, sizeof h, st);
+  int rc = rt::copy_d2h(&h, scratch + d.ctl + 1, sizeof h, st);
   if (!rc) rc = rt::stream_sync(st);
   if (rc) return rc;
   return h ? rt::E_CUDA : rt::OK;
 }
 
-// p: n coefficients, q: n-1 coefficients (n >= 1), rem: 1 element, z: 1 element; all device.
+// p: d.n coefficients, q: d.n - 1 coefficients, rem: 1 element, z: 1 element, scratch: d.words; all device.
 template <class R>
-inline int fr_div_linear(const uint32_t *p, size_t n, const uint32_t *z, uint32_t *q, uint32_t *rem,
+inline int fr_div_linear(const DivPlan &d, const uint32_t *p, const uint32_t *z, uint32_t *q, uint32_t *rem,
                          uint32_t *scratch, rt::stream_t st) {
-  if (n == 0) return rt::dev_memset(rem, 0, 32, st);
-  size_t cnt[DIV_MAX_LEVELS]; uint32_t *local[DIV_MAX_LEVELS], *carry[DIV_MAX_LEVELS];
-  uint32_t *zp = scratch, *cur = scratch + 8 * DIV_MAX_LEVELS;
-  int levels = 0;
-  for (size_t c = (n + DIV_K - 1) / DIV_K;; c = (c + DIV_F - 1) / DIV_F) {
-    cnt[levels] = c; local[levels] = cur; cur += 8 * c; carry[levels] = cur; cur += 8 * c;
-    levels++;
-    if (c <= DIV_F || levels == DIV_MAX_LEVELS) break;
-  }
+  const size_t n = d.n;
   int rc;
-  // one pass up to 2^21 coefficients; beyond that the level tree's fewer products per coefficient win;
-  // PCGPU_DIV_MODE = tile | tree forces one
-  if (div_one_pass(n)) {
+  if (d.path == DIV_PATH_NONE) return rt::dev_memset(rem, 0, 32, st);
+  if (d.path == DIV_PATH_TILES) {
     // one pass: powers (one small launch), control words cleared, tiles chained by a decoupled look-back
-    const uint32_t ntiles = (uint32_t)((n + DIVT_TILE - 1) / DIVT_TILE);
-    uint32_t *pw = scratch, *aggp = pw + 8 * DIVT_POW_COUNT, *incp = aggp + 8 * (size_t)ntiles, *ctl = incp + 8 * (size_t)ntiles;
-    if ((rc = rt::dev_memset(ctl, 0, (2 + (size_t)ntiles) * 4, st))) return rc;
+    uint32_t *pw = scratch, *ctl = scratch + d.ctl;
+    if ((rc = rt::dev_memset(ctl, 0, (2 + (size_t)d.ntiles) * 4, st))) return rc;
     if ((rc = rt::launch<64>(DivTilePowersBody<R>{z, pw}, DIVT_POW_COUNT, st))) return rc;
-    return rt::launch_blocks<DIVT_THREADS>(DivTileBody<R>{p, n, z, pw, q, rem, ctl, aggp, incp, ntiles}, ntiles, divt_smem_bytes(), st);
+    return rt::launch_blocks<DIVT_THREADS>(DivTileBody<R>{p, n, z, pw, q, rem, ctl, scratch + d.agg, scratch + d.inc, d.ntiles},
+                                           d.ntiles, divt_smem_bytes(), st);
   }
-  // (a three-launch variant with ONE block scanning all chunk carries has 128 dependent products per thread twice over;
-  // the level tree below keeps every chain at DIV_F = 32)
-  if (getenv("PCGPU_DIV_BLOCK_SCAN") && cnt[0] <= (size_t)DIV_SCAN_BLOCK * 4096) {
-    if ((rc = rt::launch<128>(DivChunkLocalBody<R>{p, n, z, local[0]}, cnt[0], st))) return rc;
-    if ((rc = rt::launch_blocks<DIV_SCAN_BLOCK>(DivBlockScanBody<R>{local[0], cnt[0], z, carry[0], rem}, 1, (16 * DIV_SCAN_BLOCK + 32) * 4, st))) return rc;
-    return rt::launch<128>(DivChunkWriteBody<R>{p, n, z, carry[0], q}, cnt[0], st);
-  }
+  const int levels = d.levels;
+  const size_t *cnt = d.cnt;
+  uint32_t *zp = scratch, *local[DIV_MAX_LEVELS], *carry[DIV_MAX_LEVELS];
+  for (int l = 0; l < levels; l++) { local[l] = scratch + d.local[l]; carry[l] = scratch + d.carry[l]; }
   if ((rc = rt::launch<32>(DivPowersBody<R>{z, zp, (uint32_t)levels}, 1, st))) return rc;
   if ((rc = rt::launch<128>(DivChunkLocalBody<R>{p, n, z, local[0]}, cnt[0], st))) return rc;
   for (int l = 1; l < levels; l++)

@@ -809,21 +809,22 @@ int fr_div_impl(pcgpu_ctx *ctx, const void *p, size_t n, const void *z, void *q,
   rt::stream_t st = ctx->stream;
   int rc;
   const uint32_t *d_z, *d_p; uint32_t *d_rem, *scratch, *d_q;
+  const DivPlan plan = div_plan(n);
   Staging io(ctx, flags);
   io.host_in(d_z, z, 32);
   io.scratch(d_rem, 32);
-  io.scratch(scratch, div_scratch_words(n) * 4);
+  io.scratch(scratch, plan.words * 4);
   io.in(d_p, p, n * 32);
   io.out(d_q, q, n > 1 ? (n - 1) * 32 : 0);
   if ((rc = io.upload())) return rc;
   ctx->prof.begin(7, st);
-  if ((rc = fr_div_linear<R>(d_p, n, d_z, d_q, d_rem, scratch, st))) return rc;
+  if ((rc = fr_div_linear<R>(plan, d_p, d_z, d_q, d_rem, scratch, st))) return rc;
   ctx->prof.end(7, st);
   if ((rc = io.download())) return rc;
   uint32_t hrem[8];
   if ((rc = rt::copy_d2h(hrem, d_rem, 32, st))) return rc;
   if ((rc = rt::stream_sync(st))) return rc;
-  if ((rc = fr_div_check(scratch, n, st))) return rc;
+  if ((rc = fr_div_check(plan, scratch, st))) return rc;
   if (rem) memcpy(rem, hrem, 32);
   ctx->prof.collect();
   return PCGPU_OK;
@@ -914,11 +915,12 @@ int kzg_open_impl(pcgpu_ctx *ctx, const pcgpu_srs *pg, const void *coeffs, size_
   rt::stream_t st = ctx->stream;
   int rc;
   const uint32_t *d_z, *d_c, *d_b; uint32_t *d_rem, *d_rv, *scratch, *d_q, *d_bq;
+  const DivPlan wp = div_plan(n), bp = div_plan(n_blind);   // the two divisions run one after the other in one scratch
   Staging io(ctx, flags);
   io.host_in(d_z, z, 32);
   io.scratch(d_rem, 32);
   io.scratch(d_rv, 32);
-  io.scratch(scratch, div_scratch_words(n > n_blind ? n : n_blind) * 4);
+  io.scratch(scratch, (wp.words > bp.words ? wp.words : bp.words) * 4);
   io.scratch(d_q, n * 32);
   io.scratch(d_bq, n_blind * 32);
   io.in(d_c, coeffs, n * 32);
@@ -926,15 +928,15 @@ int kzg_open_impl(pcgpu_ctx *ctx, const pcgpu_srs *pg, const void *coeffs, size_
   if ((rc = io.upload())) return rc;
   // witness = p / (X - z)   (kzg10/mod.rs:222-226)
   ctx->prof.begin(7, st);
-  if ((rc = fr_div_linear<R>(d_c, n, d_z, d_q, d_rem, scratch, st))) return rc;
+  if ((rc = fr_div_linear<R>(wp, d_c, d_z, d_q, d_rem, scratch, st))) return rc;
   ctx->prof.end(7, st);
   host::HXYZZ<C> w, rw;
   if ((rc = msm_to_host<C>(ctx, pg, 0, d_q, n ? n - 1 : 0, true, &w))) return rc;     // :255-258
-  if ((rc = fr_div_check(scratch, n, st))) return rc;
+  if ((rc = fr_div_check(wp, scratch, st))) return rc;
   if (n_blind) {
-    if ((rc = fr_div_linear<R>(d_b, n_blind, d_z, d_bq, d_rv, scratch, st))) return rc;  // rem = blind(z), :264
+    if ((rc = fr_div_linear<R>(bp, d_b, d_z, d_bq, d_rv, scratch, st))) return rc;  // rem = blind(z), :264
     if ((rc = msm_to_host<C>(ctx, gamma, 0, d_bq, n_blind - 1, true, &rw))) return rc;  // :270-273
-    if ((rc = fr_div_check(scratch, n_blind, st))) return rc;
+    if ((rc = fr_div_check(bp, scratch, st))) return rc;
     if (out_random_v) {
       if ((rc = rt::copy_d2h(out_random_v, d_rv, 32, st))) return rc;
       if ((rc = rt::stream_sync(st))) return rc;
@@ -1001,11 +1003,12 @@ int kzg_commit_open_impl(pcgpu_ctx *ctx, pcgpu_ctx *sib, const pcgpu_srs *pg, co
   if (n > pg->n) return PCGPU_E_DEGREE;                      // kzg10/mod.rs:163, :292
   rt::stream_t sa = ctx->stream, sb = sib->stream;
   const uint32_t *d_c, *d_z; uint32_t *d_rem, *scratch, *d_q;
+  const DivPlan plan = div_plan(n);
   Staging a(ctx, flags), b(sib, flags);   // the coefficients on ctx's stream, the witness side on sib's
   a.in(d_c, coeffs, n * 32);
   b.host_in(d_z, z, 32);
   b.scratch(d_rem, 32);
-  b.scratch(scratch, div_scratch_words(n) * 4);
+  b.scratch(scratch, plan.words * 4);
   b.scratch(d_q, n * 32);
   if ((rc = a.upload()) || (rc = b.upload())) return rc;
   if (!ctx->ev_ok) { if ((rc = rt::event_create(&ctx->ev_upload))) return rc; ctx->ev_ok = true; }
@@ -1014,14 +1017,14 @@ int kzg_commit_open_impl(pcgpu_ctx *ctx, pcgpu_ctx *sib, const pcgpu_srs *pg, co
   MsmPending<C> pc, pw;
   // witness side first: its division is short and its MSM then overlaps the commitment's
   sib->prof.begin(7, sb);
-  if ((rc = fr_div_linear<R>(d_c, n, d_z, d_q, d_rem, scratch, sb))) return rc;      // kzg10/mod.rs:222-226
+  if ((rc = fr_div_linear<R>(plan, d_c, d_z, d_q, d_rem, scratch, sb))) return rc;   // kzg10/mod.rs:222-226
   sib->prof.end(7, sb);
   if ((rc = msm_issue<C>(ctx, pg, 0, d_c, n, true, &pc))) return rc;                 // :175-178
   if ((rc = msm_issue<C>(sib, pg, 0, d_q, n ? n - 1 : 0, true, &pw))) return rc;     // :255-258
   host::HXYZZ<C> comm, w;
   if ((rc = msm_collect<C>(ctx, &pc, &comm))) return rc;
   if ((rc = msm_collect<C>(sib, &pw, &w))) return rc;
-  if ((rc = fr_div_check(scratch, n, sb))) return rc;
+  if ((rc = fr_div_check(plan, scratch, sb))) return rc;
   host::to_affine<C>(comm, out_c_xy, out_c_inf);                                      // :209
   host::to_affine<C>(w, out_w_xy, out_w_inf);                                         // :281
   return PCGPU_OK;
@@ -1054,20 +1057,16 @@ static int ensure_pow2(pcgpu_ctx *ctx) {
   return rt::launch<32>(Pow2TableBody<QP>{ctx->d_pow2[C::ID]}, 1, ctx->stream);
 }
 
-#ifndef PCGPU_IPA_FOLD_MIN_BLOCKS
-#define PCGPU_IPA_FOLD_MIN_BLOCKS 2
-#endif
-enum { IPA_FOLD_MIN_BLOCKS = PCGPU_IPA_FOLD_MIN_BLOCKS };
-// freeze the key at its current length (<= SMALL_MAX_N): weights start at one
+// freeze the key at its current length once that is 2 .. SMALL_MAX_N points (unless PCGPU_IPA_FREEZE=0 or the small MSM is
+// off): weights start at one.  Called after every change of the key's length.
 template <class C>
-static int ipa_freeze(pcgpu_ctx *ctx, pcgpu_ipa *st) {
+static int ipa_maybe_freeze(pcgpu_ctx *ctx, pcgpu_ipa *st) {
   using R = typename C::Fr;
+  if (!(st->n <= SMALL_MAX_N && st->n > 1 && msm_small_enabled())) return PCGPU_OK;
+  const char *e = getenv("PCGPU_IPA_FREEZE");
+  if (e && e[0] == '0') return PCGPU_OK;
   st->frozen_m = st->n;
   return rt::launch<128>(FrFillOneBody<R>{st->d_w}, st->n, ctx->stream);
-}
-inline bool ipa_freeze_enabled() {
-  const char *e = getenv("PCGPU_IPA_FREEZE");
-  return msm_small_enabled() && !(e && e[0] == '0');
 }
 
 template <class C>
@@ -1097,10 +1096,11 @@ int ipa_begin_impl(pcgpu_ctx *ctx, const void *key_xy, size_t n, const void *coe
   if ((rc = rt::launch<128>(FrPowersBody<R>{st->d_point, st->d_z}, n, s))) return rc;
   st->view.curve = C::ID; st->view.n = n; st->view.c = 0; st->view.groups = 1; st->view.d_tables = st->d_key; st->view.d_folded = nullptr;
   st->view.d_comb = nullptr; st->view.comb_c = 0;
-  if (n <= SMALL_MAX_N && n > 1 && ipa_freeze_enabled() && (rc = ipa_freeze<C>(ctx, st))) return rc;
+  if ((rc = ipa_maybe_freeze<C>(ctx, st))) return rc;
   return rt::stream_sync(s);
 }
 
+// sib: the sibling context whose stream runs the second commitment of a bucket-pipeline round (never null)
 template <class C>
 int ipa_round_lr_impl(pcgpu_ctx *ctx, pcgpu_ctx *sib, pcgpu_ipa *st, const void *h_prime_xy, void *out_l_xy, uint8_t *out_l_inf,
                       void *out_r_xy, uint8_t *out_r_inf) {
@@ -1111,54 +1111,41 @@ int ipa_round_lr_impl(pcgpu_ctx *ctx, pcgpu_ctx *sib, pcgpu_ipa *st, const void 
   if (m == 0) return PCGPU_E_BADARG;
   const uint32_t *cl = st->d_coeffs, *cr = st->d_coeffs + 8 * m, *zl = st->d_z, *zr = st->d_z + 8 * m;
   uint32_t *d_ip = st->d_ip, *scr = st->d_ip_scratch;
-  const Affine<C> *d_h = (const Affine<C> *)st->d_h;
-  uint64_t ip_m[2][4], ip_c[2][4];
-  if (st->frozen_m) {
-    // frozen key: both commitments are frozen_m-term MSMs over the same points, scalars expanded on the device
-    const size_t M = st->frozen_m;
-    if ((rc = fr_inner_product<R>(cr, zl, m, d_ip, scr, s))) return rc;
-    if ((rc = fr_inner_product<R>(cl, zr, m, d_ip + 8, scr, s))) return rc;
+  const Affine<C> *d_h = (const Affine<C> *)st->d_h, *key = (const Affine<C> *)st->d_key;
+  // the round's path: a frozen key (two frozen_m-term MSMs over the same points, scalars expanded on the device), <= 8192-term
+  // commitments (the bucket pipeline's fixed cost dominates at this size: both in ONE small-MSM launch), or two bucket pipelines
+  enum { FROZEN, SMALL, BUCKETS } path = st->frozen_m ? FROZEN : m <= 2 * SMALL_MAX_N && msm_small_enabled() ? SMALL : BUCKETS;
+  // <coeffs_r, z_l>, <coeffs_l, z_r>
+  if ((rc = fr_inner_product<R>(cr, zl, m, d_ip, scr, s))) return rc;
+  if ((rc = fr_inner_product<R>(cl, zr, m, d_ip + 8, scr, s))) return rc;   // stream order: the first product is complete
+  if (path != BUCKETS) {
+    // each commitment with its  + h' * <.,.>  term in the same launch; the inner products never leave HBM
     if ((rc = rt::copy_h2d(st->d_h, h_prime_xy, sizeof(Affine<C>), s))) return rc;
-    if ((rc = rt::launch<128>(IpaFrozenScalarsBody<R>{st->d_w, st->d_coeffs, (uint32_t)st->n, st->d_sl, st->d_sr}, M, s))) return rc;
-    const Affine<C> *key = (const Affine<C> *)st->d_key;
-    MsmSmallProblem<C> pr[2] = {{key, st->d_sl, d_h, d_ip, (uint32_t)M}, {key, st->d_sr, d_h, d_ip + 8, (uint32_t)M}};
+    size_t M = m;
+    const Affine<C> *kl = key, *kr = key + m;   // cm_commit(key_l, coeffs_r), cm_commit(key_r, coeffs_l)
+    const uint32_t *sl = cr, *sr = cl;
+    if (path == FROZEN) {
+      M = st->frozen_m; kr = key; sl = st->d_sl; sr = st->d_sr;
+      if ((rc = rt::launch<128>(IpaFrozenScalarsBody<R>{st->d_w, st->d_coeffs, (uint32_t)st->n, st->d_sl, st->d_sr}, M, s))) return rc;
+    }
+    MsmSmallProblem<C> pr[2] = {{kl, sl, d_h, d_ip, (uint32_t)M}, {kr, sr, d_h, d_ip + 8, (uint32_t)M}};
     host::HXYZZ<C> lr[2];
     if ((rc = msm_small_to_host<C>(ctx, msm_small_plan(M), pr, 2, true, lr))) return rc;
     host::to_affine<C>(lr[0], out_l_xy, out_l_inf);
     host::to_affine<C>(lr[1], out_r_xy, out_r_inf);
     return PCGPU_OK;
   }
-  if (m <= 2 * SMALL_MAX_N && msm_small_enabled()) {
-    // rounds of <= 8192-term commitments (the bucket pipeline's fixed cost dominates at this size): both commitments, each with its  + h' * <.,.>  term, in ONE launch; the inner products never leave HBM
-    if ((rc = fr_inner_product<R>(cr, zl, m, d_ip, scr, s))) return rc;
-    if ((rc = fr_inner_product<R>(cl, zr, m, d_ip + 8, scr, s))) return rc;
-    if ((rc = rt::copy_h2d(st->d_h, h_prime_xy, sizeof(Affine<C>), s))) return rc;
-    const Affine<C> *key = (const Affine<C> *)st->view.d_tables;
-    MsmSmallProblem<C> pr[2] = {{key, cr, d_h, d_ip, (uint32_t)m},          // cm_commit(key_l, coeffs_r) + h' <c_r, z_l>
-                                {key + m, cl, d_h, d_ip + 8, (uint32_t)m}};  // cm_commit(key_r, coeffs_l) + h' <c_l, z_r>
-    host::HXYZZ<C> lr[2];
-    if ((rc = msm_small_to_host<C>(ctx, msm_small_plan(m), pr, 2, true, lr))) return rc;
-    host::to_affine<C>(lr[0], out_l_xy, out_l_inf);
-    host::to_affine<C>(lr[1], out_r_xy, out_r_inf);
-    return PCGPU_OK;
-  }
-  // <coeffs_r, z_l>, <coeffs_l, z_r> (results fetched after the MSMs have been queued), then the two commitments: cm_commit(key_l,
-  // coeffs_r) on this context's stream and cm_commit(key_r, coeffs_l) on the sibling's, so their latency-bound stages overlap
-  if ((rc = fr_inner_product<R>(cr, zl, m, d_ip, scr, s))) return rc;
-  if ((rc = fr_inner_product<R>(cl, zr, m, d_ip + 8, scr, s))) return rc;   // stream order: the first product is complete
+  // the inner products are copied back and their h' terms added on the host once the MSMs are done; cm_commit(key_l, coeffs_r)
+  // runs on this context's stream and cm_commit(key_r, coeffs_l) on the sibling's, so their latency-bound stages overlap
+  uint64_t ip_m[2][4], ip_c[2][4];
   if ((rc = rt::copy_d2h(ip_m[0], d_ip, 32, s))) return rc;
   if ((rc = rt::copy_d2h(ip_m[1], d_ip + 8, 32, s))) return rc;
   host::HXYZZ<C> l, r;
-  if (sib) {
-    MsmPending<C> pl, pr;
-    if ((rc = msm_issue<C>(ctx, &st->view, 0, cr, m, true, &pl))) return rc;
-    if ((rc = msm_issue<C>(sib, &st->view, m, cl, m, true, &pr))) return rc;
-    if ((rc = msm_collect<C>(ctx, &pl, &l))) return rc;
-    if ((rc = msm_collect<C>(sib, &pr, &r))) return rc;
-  } else {
-    if ((rc = msm_to_host<C>(ctx, &st->view, 0, cr, m, true, &l))) return rc;  // cm_commit(key_l, coeffs_r)
-    if ((rc = msm_to_host<C>(ctx, &st->view, m, cl, m, true, &r))) return rc;  // cm_commit(key_r, coeffs_l)
-  }
+  MsmPending<C> pl, pr;
+  if ((rc = msm_issue<C>(ctx, &st->view, 0, cr, m, true, &pl))) return rc;
+  if ((rc = msm_issue<C>(sib, &st->view, m, cl, m, true, &pr))) return rc;
+  if ((rc = msm_collect<C>(ctx, &pl, &l))) return rc;
+  if ((rc = msm_collect<C>(sib, &pr, &r))) return rc;
   if ((rc = rt::stream_sync(s))) return rc;
   host::fr_from_mont_host<R>(ip_m[0], ip_c[0]);
   host::fr_from_mont_host<R>(ip_m[1], ip_c[1]);
@@ -1187,31 +1174,28 @@ int ipa_round_fold_impl(pcgpu_ctx *ctx, pcgpu_ipa *st, const void *challenge, co
   }
   uint64_t canon[4];
   host::fr_from_mont_host<R>(challenge, canon);
-  host::GlvSplit gs;
-  gs.ok = false;
-  if (C::Fq::COFACTOR_ONE) {                       // phi acts as lambda on the whole curve only when the cofactor is 1
+  bool glv = false;
+  if constexpr (C::Fq::COFACTOR_ONE) {             // phi acts as lambda on the whole curve only when the cofactor is 1
     const char *e = getenv("PCGPU_IPA_GLV");
+    host::GlvSplit gs;
+    gs.ok = false;
     if (!(e && e[0] == '0')) gs = host::glv_decompose<C>(canon);
+    if ((glv = gs.ok)) {
+      G1FoldGlvBody<C> gb; gb.key = (Affine<C> *)st->d_key; gb.m = (uint32_t)m;
+      memcpy(gb.u1_nz, gs.u1_nz, sizeof gb.u1_nz); memcpy(gb.u1_sg, gs.u1_sg, sizeof gb.u1_sg);
+      memcpy(gb.u2_nz, gs.u2_nz, sizeof gb.u2_nz); memcpy(gb.u2_sg, gs.u2_sg, sizeof gb.u2_sg);
+      gb.neg1 = gs.neg1; gb.neg2 = gs.neg2; gb.ncols = gs.jsf_len; gb.pow2 = ctx->d_pow2[C::ID];
+      // registers: 182 (BN254) / 192 (Pallas) uncapped, 2 blocks of 128 threads per SM; 3 or 4 resident blocks would cap them at 168 / 128
+      if ((rc = rt::launch<128>(gb, m, s))) return rc;                                                      // :699-707
+    }
   }
-  if (gs.ok) {
-    G1FoldGlvBody<C> gb; gb.key = (Affine<C> *)st->d_key; gb.m = (uint32_t)m;
-    memcpy(gb.u1_nz, gs.u1_nz, sizeof gb.u1_nz); memcpy(gb.u1_sg, gs.u1_sg, sizeof gb.u1_sg);
-    memcpy(gb.u2_nz, gs.u2_nz, sizeof gb.u2_nz); memcpy(gb.u2_sg, gs.u2_sg, sizeof gb.u2_sg);
-    gb.neg1 = gs.neg1; gb.neg2 = gs.neg2; gb.ncols = gs.jsf_len; gb.pow2 = ctx->d_pow2[C::ID];
-    // registers: 190 uncapped (2 blocks of 128 threads per SM); 3 or 4 resident blocks cap them at 168 / 128 (PCGPU_IPA_FOLD_OCC)
-    int occ = IPA_FOLD_MIN_BLOCKS;
-    if (const char *e = getenv("PCGPU_IPA_FOLD_OCC")) { int v = atoi(e); if (v >= 2 && v <= 4) occ = v; }
-    if (occ == 2) rc = rt::launch<128>(gb, m, s);
-    else if (occ == 3) rc = rt::launch_occ<128, 3>(gb, m, s);
-    else rc = rt::launch_occ<128, 4>(gb, m, s);
-    if (rc) return rc;                                                                                      // :699-707
-  } else {
+  if (!glv) {
     G1FoldBody<C> fb; fb.key = (Affine<C> *)st->d_key; fb.m = (uint32_t)m;
     memcpy(fb.chal, canon, 32); fb.pow2 = ctx->d_pow2[C::ID];
     if ((rc = rt::launch<128>(fb, m, s))) return rc;                                                        // :699-707
   }
   st->n = m; st->view.n = m;
-  if (m <= SMALL_MAX_N && m > 1 && ipa_freeze_enabled() && (rc = ipa_freeze<C>(ctx, st))) return rc;
+  if ((rc = ipa_maybe_freeze<C>(ctx, st))) return rc;
   return rt::stream_sync(s);
 }
 

@@ -464,7 +464,7 @@ def test_concurrent_host_threads(eng, pc):
 
 def test_randomised_sweep(capsys):
     """A short run of tests/perf/fuzz_gpu.py (random shapes across the small-path / split / bucket-pipeline boundaries, scalar
-    mixtures, base offsets, the three division modes, NTT + inverse, hiding commits / opens), bit-exact against the C oracle."""
+    mixtures, base offsets, both division paths, NTT + inverse, hiding commits / opens), bit-exact against the C oracle."""
     import importlib.util
     import os
     import sys

@@ -547,14 +547,12 @@ def test_fixed_base_mul(eng, cname):
 
 
 @pytest.mark.parametrize("cname", util.CURVE_NAMES)
-@pytest.mark.parametrize("n,mode", [(1, "tile"), (2, "tile"), (31, "tree"), (32, "tile"), (33, "scan"), (2048, "tile"), (2049, "tile"),
-                                    (2049, "tree"), (5000, "tree"), (6145, "tile"), (70001, "scan"), (70001, "tile"), (70001, "tree")])
+@pytest.mark.parametrize("n,mode", [(1, "tile"), (2, "tile"), (31, "tree"), (32, "tile"), (33, "tree"), (2048, "tile"), (2049, "tile"),
+                                    (2049, "tree"), (5000, "tree"), (6145, "tile"), (70001, "tile"), (70001, "tree")])
 def test_fr_div_linear(eng, cname, n, mode, monkeypatch):
     # tile: the one-pass kernel (tiles chained by a decoupled look-back; the default up to 2^21 coefficients), tree: the level
-    # tree (the default beyond), scan: the one-block carry scan (kept as an experiment knob)
-    monkeypatch.setenv("PCGPU_DIV_MODE", "tile" if mode == "tile" else "tree")
-    if mode == "scan":
-        monkeypatch.setenv("PCGPU_DIV_BLOCK_SCAN", "1")
+    # tree (the default beyond)
+    monkeypatch.setenv("PCGPU_DIV_MODE", mode)
     C = pyref.Curve(cname)
     p = util.rand_fr(cname, n, seed=20 + n, mont=True)
     z = util.rand_fr(cname, 1, seed=21, mont=True)[0]
