@@ -54,15 +54,19 @@ def round_transcript(eng, curve, round_challenge, l, l_inf, r, r_inf):
     return int(round_challenge).to_bytes(32, "little") + enc.tobytes()
 
 
-def open_rounds(eng, curve, comm_key_xy, coeffs, point, h_prime_xy, round_challenge):
+def open_rounds(eng, curve, comm_key_xy, coeffs, point, h_prime_xy, round_challenge, n=None, flags=0, n_coeffs=None,
+                on_round=None):
     """The `while n > 1` loop (:665-711).  comm_key_xy: n affine points; coeffs: <= n Montgomery Fr; point: Montgomery
-    Fr; h_prime_xy: affine h' = h * round_challenge (:631); round_challenge: the initial challenge as an int.
-    Returns dict(l_vec, r_vec, final_comm_key, c, challenges)."""
+    Fr; h_prime_xy: affine h' = h * round_challenge (:631); round_challenge: the initial challenge as an int.  n, flags,
+    n_coeffs: as Engine.ipa_begin (device-resident key and coefficients with DEVICE_PTRS).  on_round(t): called after
+    round t's l and r are computed, before its fold.  Returns dict(l_vec, r_vec, final_comm_key, c, challenges)."""
     r = _MODULI[curve]
-    st = eng.ipa_begin(curve, comm_key_xy, coeffs, point)
+    st = eng.ipa_begin(curve, comm_key_xy, coeffs, point, n=n, flags=flags, n_coeffs=n_coeffs)
     l_vec, r_vec, chals = [], [], []
     while eng.ipa_len(st) > 1:
         l, l_inf, rr, r_inf = eng.ipa_round_lr(curve, st, h_prime_xy, with_inf=True)
+        if on_round:
+            on_round(len(l_vec))
         l_vec.append(l)
         r_vec.append(rr)
         data = round_transcript(eng, curve, round_challenge, l, l_inf, rr, r_inf)          # :681-687

@@ -7,7 +7,7 @@ The policy restated here is the one csrc/impl.cuh msm_plan decides (with csrc/ms
 csrc/srs.cuh srs_precompute_window); it is the suite's only copy, G2 cases (tests/g2_cases.py) included:
   * n = 0: no MSM (path NONE, every word 0);
   * n <= SMALL_MAX_N with PCGPU_MSM_SMALL unset or not "0": the one-launch kernel, split = 1 block per window below 512 terms,
-    else 3;
+    else 3; the IPA's two-problem launch (csrc/impl.cuh msm_small_plan) also takes it for 4097 ... 8192 terms, split = 6;
   * window-folded tables (SRS_PRECOMPUTE, n >= 4096): c = the registration's window, G = W table groups, one bucket set;
   * raw bases: c = clamp(floor(log2 n) - 4, 8, 16) or PCGPU_MSM_C, G = 1, S = W bucket sets;
   * W = ceil(bits(r) / c); entries = n * W; buckets TB = S * 2^(c-1);
@@ -27,6 +27,7 @@ SRS_PRECOMPUTE_MIN_N = 1 << 12
 SMALL_MAX_N = 4096              # csrc/msm_small.cuh: the one-launch kernel's largest problem
 SMALL_SPLIT_MIN_N = 512         # csrc/msm_small.cuh: from this many terms a window is split over SMALL_SPLIT blocks
 SMALL_SPLIT = 3
+SMALL_WIDE_MAX_N = 2 * SMALL_MAX_N   # the IPA's l / r commitments: the one-launch kernel up to this many terms, 6 blocks per window
 HEAVY_BUCKET_TASKS = 8          # csrc/msm.cuh: a bucket with more accumulate tasks than this goes to MsmHeavyBucketBody
 HEAVY_GRID = 64                 # blocks of MsmHeavyBucketBody (grid-strided over the heavy list)
 DEPTH_SLOTS = 32                # a "depth" case gives every pair-round thread at least this many round-0 slots
@@ -46,6 +47,11 @@ def srs_precompute_window(n):
     return 17 if lg >= 18 else 14 if lg >= 15 else 12
 
 
+def small_split(n):
+    """blocks per window of the one-launch kernel for problems of n terms (csrc/impl.cuh msm_small_plan)"""
+    return 2 * SMALL_SPLIT if n > SMALL_MAX_N else SMALL_SPLIT if n >= SMALL_SPLIT_MIN_N else 1
+
+
 def policy_rounds(entries, tb, wave):
     avg, r = entries // tb, 0
     while r < 8 and (avg >> r) >= 4 and (entries >> (r + 1)) >= 16 * wave:
@@ -58,19 +64,18 @@ def pair_threads(wave, tdiv):
     return t if tdiv == 1 else (t // tdiv + 127) // 128 * 128
 
 
-def check_geometry(eng, pc, cname, n, folded_c=None, tdiv=1, depth=False, g2=False, small=False):
+def check_geometry(eng, pc, cname, n, folded_c=None, tdiv=1, depth=False, g2=False, small=False, small_max=SMALL_MAX_N):
     """asserts every word of the report of the last MSM on `eng`, an MSM of n terms.  n = 0 took no path; with small (the
-    one-launch kernel enabled) n <= SMALL_MAX_N took it; every other MSM took the bucket pipeline with the documented
-    geometry.  folded_c: the window the SRS_PRECOMPUTE tables were registered with (None: raw bases).  tdiv: the pair-round
+    one-launch kernel enabled) n <= small_max took it (SMALL_WIDE_MAX_N for an IPA round); every other MSM took the bucket
+    pipeline with the documented geometry.  folded_c: the window the SRS_PRECOMPUTE tables were registered with (None: raw bases).  tdiv: the pair-round
     divisor expected without a PCGPU_MSM_AFFINE_TDIV knob.  depth: the pair rounds must run and give every thread
     >= DEPTH_SLOTS round-0 slots.  g2: a G2 MSM (raw bases, no pair rounds).  Returns the report."""
     g = eng.msm_last_geometry()
     if n == 0:
         assert g == dict.fromkeys(g, 0), g
         return g
-    if small and n <= SMALL_MAX_N:
-        split = SMALL_SPLIT if n >= SMALL_SPLIT_MIN_N else 1
-        assert g == dict(dict.fromkeys(g, 0), path=pc.binding.MSM_PATH_SMALL, n=n, split=split), g
+    if small and n <= small_max:
+        assert g == dict(dict.fromkeys(g, 0), path=pc.binding.MSM_PATH_SMALL, n=n, split=small_split(n)), g
         return g
     bits = pyref.Curve(cname).r.bit_length()
     assert g["path"] == pc.binding.MSM_PATH_BUCKETS and g["n"] == n and g["split"] == 0, g

@@ -298,51 +298,6 @@ def test_cfg4_hyrax_commit_rows(eng, pc):
         assert (lt[cidx] == orc.fr_inner_product(C.id, l, col)).all()
 
 
-def test_cfg3_ipa_open_2p18_pallas(eng, pc):
-    """BASELINE.json cfg3: InnerProductArgPC open, degree 2^18 - 1, Pallas: the whole 18-round loop on the device;
-    parity through (i) round-1 l and r against the oracle directly, (ii) the closed forms of the loop:
-    c = sum_i coeffs[i] * prod_j inv_j^{b_j(i)},  final_comm_key = sum_i (prod_j chal_j^{b_j(i)}) key[i]."""
-    from poly_commit_b200 import ipa_pc
-    cname = "pallas"
-    C = pyref.Curve(cname)
-    logn = 18
-    n = 1 << logn
-    key = gpu_srs(eng, cname, n, seed=40)
-    h_prime = util.random_points(cname, 1, seed=41)[0]
-    coeffs = util.rand_fr_fast(cname, n, seed=42)
-    point = util.rand_fr(cname, 1, seed=43, mont=True)[0]
-    got = ipa_pc.open_rounds(eng, C.id, key, coeffs, point, h_prime, 0xabcdef)
-    assert len(got["l_vec"]) == logn
-    # (i) first round against the oracle
-    m = n // 2
-    z_int = C.fr_from_limbs(point, True)[0]
-    co_int = C.fr_from_limbs(coeffs, True)
-    zp = [1] * n
-    for i in range(1, n):
-        zp[i] = zp[i - 1] * z_int % C.r
-    def cm(keypart, sc_ints, ip):
-        msm, inf = orc.msm(C.id, keypart, C.fr_to_limbs(sc_ints, False))
-        hp, hinf = orc.g1_mul(C.id, h_prime, C.fr_to_limbs([ip], False))
-        return orc.g1_sum(C.id, np.stack([msm, hp]), inf=np.array([inf, hinf], dtype=np.uint8))[0]
-    l0 = cm(key[:m], co_int[m:], sum(a * b for a, b in zip(co_int[m:], zp[:m])) % C.r)
-    r0 = cm(key[m:], co_int[:m], sum(a * b for a, b in zip(co_int[:m], zp[m:])) % C.r)
-    assert (got["l_vec"][0] == l0).all() and (got["r_vec"][0] == r0).all()
-    # (ii) closed forms
-    ch = got["challenges"]
-    inv = [pow(c, -1, C.r) for c in ch]
-    s_ch, s_inv = [1], [1]
-    for j in range(logn - 1, -1, -1):          # last round pairs neighbours (lowest bit), first round the top bit
-        s_ch = s_ch + [x * ch[j] % C.r for x in s_ch]
-        s_inv = s_inv + [x * inv[j] % C.r for x in s_inv]
-    c_exp = sum(a * b for a, b in zip(co_int, s_inv)) % C.r
-    assert C.fr_from_limbs(got["c"], True)[0] == c_exp
-    fk = orc.msm(C.id, key, C.fr_to_limbs(s_ch, False))
-    assert (got["final_comm_key"] == fk[0]).all()
-    # the verifier's linear-time step on the device (check_poly.compute_coeffs() + cm_commit, ipa_pc/mod.rs:760-766)
-    vk = ipa_pc.check_final_key(eng, C.id, key, ch)
-    assert (vk[0] == got["final_comm_key"]).all()
-
-
 def test_cpp_host_mirror(tmp_path):
     """poly-commit_b200/host/pcgpu.hpp (C++ mirror of kzg10::KZG10::{commit, open}, Powers, Error) driven by the compiled
     tests/cpp/host_mirror_test -- the shape of kzg10/mod.rs:546-575 end_to_end_test_template -- against the oracle."""

@@ -3,6 +3,7 @@ schedule, digit recoding, bucket bookkeeping, scans and the C-ABI host logic, ea
 or the Python big-integer oracle.  These do not replace the GPU parity tests (tests/test_gpu_*.py); they
 catch logic errors before GPU time is spent."""
 import ctypes
+import os
 
 import numpy as np
 import pytest
@@ -588,28 +589,38 @@ def test_golden_vectors(eng, cname, msm_path):
     golden_cases.check_wire_engine(eng, cname)
 
 
+def _oracle_fold(cid, key, n, chal):
+    """orc.g1_fold of key[:n] (key_l + chal * key_r), in chunks on every core (each chunk is an independent fold)"""
+    from concurrent.futures import ThreadPoolExecutor
+    m = n // 2
+    step = max(256, -(-m // (4 * (os.cpu_count() or 1))))
+    parts = [np.concatenate([key[a:min(a + step, m)], key[m + a:m + min(a + step, m)]]) for a in range(0, m, step)]
+    with ThreadPoolExecutor(os.cpu_count() or 1) as ex:
+        return np.concatenate(list(ex.map(lambda p: orc.g1_fold(cid, p, chal), parts)))
+
+
 def oracle_ipa_rounds(cname, comm_key, coeffs, point, h_prime, round_challenge):
-    """InnerProductArgPC::open's halving loop (ipa_pc/mod.rs:665-711) restated over the C oracle's primitives."""
-    from poly_commit_b200 import ipa_pc
+    """InnerProductArgPC::open's halving loop (ipa_pc/mod.rs:665-711) restated over the C oracle's primitives.  Returns
+    l_vec / r_vec with their infinity flags (l_inf / r_inf), final_comm_key, c and the round challenges it derived."""
     C = pyref.Curve(cname)
     n = comm_key.shape[0]
     co = np.zeros((n, 4), dtype=np.uint64); co[: coeffs.shape[0]] = coeffs
     z_int = C.fr_from_limbs(point, True)[0]
     z = C.fr_to_limbs([pow(z_int, i, C.r) for i in range(n)], True)
     key = comm_key.copy()
-    l_vec, r_vec = [], []
+    l_vec, r_vec, l_inf, r_inf, chals = [], [], [], [], []
     while n > 1:
         m = n // 2
         def cm(keypart, sc, ip):
             msm, inf = orc.msm(C.id, keypart, orc.field_unop("orc_fr_from_mont", C.id, sc))
             hp, hinf = orc.g1_mul(C.id, h_prime, orc.field_unop("orc_fr_from_mont", C.id, ip.reshape(1, 4)))
             return orc.g1_sum(C.id, np.stack([msm, hp]), inf=np.array([inf, hinf], dtype=np.uint8))
-        l, l_inf = cm(key[:m], co[m:n], orc.fr_inner_product(C.id, co[m:n], z[:m]))
-        r, r_inf = cm(key[m:n], co[:m], orc.fr_inner_product(C.id, co[:m], z[m:n]))
-        l_vec.append(l); r_vec.append(r)
+        l, li = cm(key[:m], co[m:n], orc.fr_inner_product(C.id, co[m:n], z[:m]))
+        r, ri = cm(key[m:n], co[:m], orc.fr_inner_product(C.id, co[:m], z[m:n]))
+        l_vec.append(l); r_vec.append(r); l_inf.append(li); r_inf.append(ri)
         # the reference's transcript, built independently of the device encoder: canonical LE scalar, then ark-serialize's
         # uncompressed encodings of l and r (oracle/pyref.py; an identity l or r carries the infinity flag)
-        pts = C.points_from_limbs(np.stack([l, r]), inf=[l_inf, r_inf])
+        pts = C.points_from_limbs(np.stack([l, r]), inf=[li, ri])
         data = int(round_challenge).to_bytes(32, "little") + pyref.g1_serialize(C, pts, False)
         digest_i = 0
         while True:                                                   # compute_random_oracle_challenge, ipa_pc/mod.rs:74-87
@@ -619,12 +630,13 @@ def oracle_ipa_rounds(cname, comm_key, coeffs, point, h_prime, round_challenge):
                 break
             digest_i += 1
         round_challenge = v
+        chals.append(v)
         inv = pow(round_challenge, -1, C.r)
         co[:m] = orc.fr_axpy(C.id, co[:m], C.fr_to_limbs([inv], True)[0], co[m:n])
         z[:m] = orc.fr_axpy(C.id, z[:m], C.fr_to_limbs([round_challenge], True)[0], z[m:n])
-        key[:m] = orc.g1_fold(C.id, key[:n], C.fr_to_limbs([round_challenge], False))
+        key[:m] = _oracle_fold(C.id, key, n, C.fr_to_limbs([round_challenge], False))
         n = m
-    return dict(l_vec=l_vec, r_vec=r_vec, final_comm_key=key[0], c=co[0])
+    return dict(l_vec=l_vec, r_vec=r_vec, l_inf=l_inf, r_inf=r_inf, final_comm_key=key[0], c=co[0], challenges=chals)
 
 
 @pytest.mark.parametrize("cname,n", [("pallas", 64), ("bls12_381", 16), ("bn254", 32),
