@@ -82,6 +82,8 @@ int pcgpu_profile_enable(pcgpu_ctx *ctx, int enable);
 int pcgpu_profile_get(pcgpu_ctx *ctx, int stage, double *ms, uint64_t *count);
 
 /* ---- SRS / committer key ---------------------------------------------------------------------- */
+/* The four creators -- pcgpu_srs_register, pcgpu_mlpc_register, pcgpu_brakedown_register, pcgpu_ipa_begin -- set *out to
+ * NULL whenever out is non-NULL, whatever they return, and store the new handle in it only on PCGPU_OK. */
 /* Upload n affine bases once (kzg10 Powers::powers_of_g, data_structures.rs:124-129; ipa CommitterKey::comm_key;
  * hyrax com_key).  inf may be NULL (no identity points).  `curve` may be a G2 group id: the key then holds raw G2 bases
  * (PCGPU_SRS_PRECOMPUTE and PCGPU_SRS_COMB return PCGPU_E_BADARG) and pcgpu_msm over it is
@@ -291,7 +293,10 @@ int pcgpu_msm_peer(pcgpu_ctx *ctx, const pcgpu_srs *srs, size_t base_offset, con
 /* ---- InnerProductArgPC::open halving loop, device-resident (ipa_pc/mod.rs:636-711) ------------------------- */
 typedef struct pcgpu_ipa pcgpu_ipa;
 /* Upload the committer key (n = d+1 affine points, n a power of two) and the combined polynomial's coefficients
- * (n_coeffs <= n Montgomery Fr, zero-padded :636-641); build z = [1, point, point^2, ...] on the device (:643-648). */
+ * (n_coeffs <= n Montgomery Fr, zero-padded :636-641); build z = [1, point, point^2, ...] on the device (:643-648).
+ * One open at a time per context: PCGPU_E_BADARG while another open begun on ctx is not finished.  The state belongs to
+ * ctx: pcgpu_ipa_round_lr, pcgpu_ipa_round_fold and pcgpu_ipa_finish return PCGPU_E_BADARG for any other context and
+ * leave the state as it was (a rejected finish does not release it). */
 int pcgpu_ipa_begin(pcgpu_ctx *ctx, int curve, const void *comm_key_xy, size_t n, const void *coeffs, size_t n_coeffs,
                     const void *point, uint32_t flags, pcgpu_ipa **out);
 /* One round, first half (:671-677): l = cm_commit(key_l, coeffs_r) + h' * <coeffs_r, z_l>,

@@ -14,7 +14,7 @@ G2_OF = {BLS12_381: BLS12_381_G2, BN254: BN254_G2}
 GEOM_FIELDS = ("path", "split", "n", "c", "W", "G", "R", "T", "tdiv", "wave", "entries", "heavy")
 MSM_PATH_NONE, MSM_PATH_SMALL, MSM_PATH_BUCKETS, MSM_PATH_COMB = 0, 1, 2, 3
 SCALARS_MONT, DEVICE_PTRS, SRS_PRECOMPUTE, NTT_INVERSE, SRS_COMB, WIRE_COMPRESSED, WIRE_NO_VALIDATE = 1, 2, 4, 8, 16, 32, 64
-E_INVALID = -8
+E_BADARG, E_INVALID = -3, -8
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 
@@ -169,7 +169,24 @@ def _u64(a):
     return np.ascontiguousarray(a, dtype=np.uint64)
 
 
-class Srs:
+class _Handle:
+    """A library handle owned by an Engine.  release() (or garbage collection) frees it once: the handle is cleared before
+    _free(ctx) runs, with ctx the engine's context, or None once the engine is closed."""
+    handle = None
+
+    def release(self):
+        h, self.handle = self.handle, None
+        if h is not None:
+            self._free(h, getattr(self.engine, "ctx", None))
+
+    def __del__(self):
+        try:
+            self.release()
+        except Exception:
+            pass
+
+
+class Srs(_Handle):
     """Device-resident bases (kzg10 Powers::powers_of_g / powers_of_gamma_g, ipa comm_key, hyrax com_key)."""
 
     def __init__(self, engine, handle, curve, n):
@@ -178,35 +195,19 @@ class Srs:
     def __len__(self):
         return self.n
 
-    def release(self):
-        if self.handle is not None:
-            self.engine.lib.pcgpu_srs_release(self.engine.ctx, self.handle)
-            self.handle = None
-
-    def __del__(self):
-        try:
-            self.release()
-        except Exception:
-            pass
+    def _free(self, h, ctx):          # no context: the library frees at once
+        self.engine.lib.pcgpu_srs_release(ctx, h)
 
 
-class BrakedownCode:
+class BrakedownCode(_Handle):
     """Device-resident code of a BrakedownPCParams (its 2L sparse matrices); m / m_ext are the row lengths before and after
     encoding."""
 
     def __init__(self, engine, handle, curve, m, m_ext):
         self.engine, self.handle, self.curve, self.m, self.m_ext = engine, handle, curve, m, m_ext
 
-    def release(self):
-        if self.handle is not None and getattr(self.engine, "ctx", None):
-            h, self.handle = self.handle, None
-            self.engine.lib.pcgpu_brakedown_release(self.engine.ctx, h)
-
-    def __del__(self):
-        try:
-            self.release()
-        except Exception:
-            pass
+    def _free(self, h, ctx):
+        self.engine.lib.pcgpu_brakedown_release(ctx, h)
 
 
 def _csc_arrays(mat):
@@ -216,25 +217,17 @@ def _csc_arrays(mat):
             np.ascontiguousarray(np.asarray(val, dtype=np.uint64).reshape(-1, 4)))
 
 
-class MlpcKey:
+class MlpcKey(_Handle):
     """Device-resident G2 half of a MultilinearPC CommitterKey: the pair-folded powers_of_h of every level."""
 
     def __init__(self, engine, handle, curve, nv):
         self.engine, self.handle, self.curve, self.nv = engine, handle, curve, nv
 
-    def release(self):
-        if self.handle is not None and getattr(self.engine, "ctx", None):
-            h, self.handle = self.handle, None
-            self.engine.lib.pcgpu_mlpc_release(self.engine.ctx, h)
-
-    def __del__(self):
-        try:
-            self.release()
-        except Exception:
-            pass
+    def _free(self, h, ctx):
+        self.engine.lib.pcgpu_mlpc_release(ctx, h)
 
 
-class DeviceBuffer:
+class DeviceBuffer(_Handle):
     """`count` Fr elements (32 bytes each) on the engine's device; `ptr(i)` is the device pointer of element i, to be passed
     with DEVICE_PTRS.  Freed on release() / garbage collection."""
 
@@ -242,56 +235,42 @@ class DeviceBuffer:
         self.engine, self.count = engine, count
         p = _vp()
         engine._ck(engine.lib.pcgpu_buf_alloc(engine.ctx, max(count, 1) * 32, ctypes.byref(p)))
-        self.base = int(p.value)
+        self.handle = int(p.value)
 
     def ptr(self, i=0):
-        return self.base + 32 * i
+        return self.handle + 32 * i
 
     def write(self, arr, at=0):
         arr = np.ascontiguousarray(arr, dtype=np.uint64).reshape(-1, 4)
         if at + arr.shape[0] > self.count:
             raise ValueError("write beyond the buffer")
-        self.engine._ck(self.engine.lib.pcgpu_buf_write(self.engine.ctx, _vp(self.base), 32 * at, _ptr(arr), arr.shape[0] * 32))
+        self.engine._ck(self.engine.lib.pcgpu_buf_write(self.engine.ctx, _vp(self.handle), 32 * at, _ptr(arr), arr.shape[0] * 32))
 
     def read(self, at=0, count=None):
         count = self.count - at if count is None else count
         out = np.zeros((count, 4), dtype=np.uint64)
-        self.engine._ck(self.engine.lib.pcgpu_buf_read(self.engine.ctx, _vp(self.base), 32 * at, _ptr(out), count * 32))
+        self.engine._ck(self.engine.lib.pcgpu_buf_read(self.engine.ctx, _vp(self.handle), 32 * at, _ptr(out), count * 32))
         return out
 
     def zero(self, at=0, count=None):
         count = self.count - at if count is None else count
-        self.engine._ck(self.engine.lib.pcgpu_buf_zero(self.engine.ctx, _vp(self.base), 32 * at, count * 32))
+        self.engine._ck(self.engine.lib.pcgpu_buf_zero(self.engine.ctx, _vp(self.handle), 32 * at, count * 32))
 
-    def release(self):
-        if getattr(self, "base", None) and getattr(self.engine, "ctx", None):
-            b, self.base = self.base, None
-            self.engine.lib.pcgpu_buf_free(self.engine.ctx, _vp(b))
-
-    def __del__(self):
-        try:
-            self.release()
-        except Exception:
-            pass
+    def _free(self, h, ctx):          # pcgpu_buf_free needs a live context
+        if ctx:
+            self.engine.lib.pcgpu_buf_free(ctx, _vp(h))
 
 
-class IpaState:
+class IpaState(_Handle):
     """Device-resident state of one InnerProductArgPC::open halving loop; released by ipa_finish, by release() or when the
     object is dropped (an exception between ipa_begin and ipa_finish therefore does not leak device memory)."""
 
     def __init__(self, engine, handle, curve):
         self.engine, self.handle, self.curve = engine, handle, curve
 
-    def release(self):
-        if self.handle is not None and getattr(self.engine, "ctx", None):
-            h, self.handle = self.handle, None
-            self.engine.lib.pcgpu_ipa_finish(self.engine.ctx, h, None, None)
-
-    def __del__(self):
-        try:
-            self.release()
-        except Exception:
-            pass
+    def _free(self, h, ctx):          # pcgpu_destroy released the IPA arena of a closed engine
+        if ctx:
+            self.engine.lib.pcgpu_ipa_finish(ctx, h, None, None)
 
 
 class Engine:
@@ -752,9 +731,16 @@ class Engine:
                                           ctypes.byref(h)))
         return IpaState(self, h, curve)
 
+    @staticmethod
+    def _ipa_curve(curve, state):
+        """the library writes points of the state's curve; `curve` must name it"""
+        if curve != state.curve:
+            raise ValueError(f"curve {curve} differs from the IPA state's curve {state.curve}")
+        return state.curve
+
     def ipa_round_lr(self, curve, state, h_prime_xy, with_inf=False):
         h_prime_xy = _u64(h_prime_xy)
-        nq = fq_limbs(curve)
+        nq = fq_limbs(self._ipa_curve(curve, state))
         l, r = np.zeros(2 * nq, dtype=np.uint64), np.zeros(2 * nq, dtype=np.uint64)
         li, ri = np.zeros(1, dtype=np.uint8), np.zeros(1, dtype=np.uint8)
         self._ck(self.lib.pcgpu_ipa_round_lr(self.ctx, state.handle, _ptr(h_prime_xy), _ptr(l), _ptr(li), _ptr(r), _ptr(ri)))
@@ -777,9 +763,11 @@ class Engine:
 
     def ipa_finish(self, curve, state):
         """final_comm_key and c; releases the device state"""
-        key, c = np.zeros(2 * fq_limbs(curve), dtype=np.uint64), np.zeros(4, dtype=np.uint64)
-        h, state.handle = state.handle, None            # pcgpu_ipa_finish frees the state whatever it returns
-        self._ck(self.lib.pcgpu_ipa_finish(self.ctx, h, _ptr(key), _ptr(c)))
+        key, c = np.zeros(2 * fq_limbs(self._ipa_curve(curve, state)), dtype=np.uint64), np.zeros(4, dtype=np.uint64)
+        rc = self.lib.pcgpu_ipa_finish(self.ctx, state.handle, _ptr(key), _ptr(c))
+        if rc != E_BADARG:          # a finish that ran frees the state whatever it returns; a rejected one leaves it open
+            state.handle = None
+        self._ck(rc)
         return key, c
 
     # ---- KZG10 ----

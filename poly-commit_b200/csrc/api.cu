@@ -29,22 +29,42 @@ static int on_ctx(pcgpu_ctx *ctx, bool bad_args, F f) {
 // x || y of one affine point of the curve (Montgomery limbs)
 static size_t affine_bytes(int curve) { return (curve == PCGPU_BLS12_381 ? 6 : 4) * 16; }
 
-static void srs_free(pcgpu_srs *srs) {
-  rt::dev_free(srs->d_tables); rt::dev_free(srs->d_folded); rt::dev_free(srs->d_comb);
+// the device memory a handle owns (an IPA state's lives in its context's arena)
+static void free_device(pcgpu_srs *srs) { rt::dev_free(srs->d_tables); rt::dev_free(srs->d_folded); rt::dev_free(srs->d_comb); }
+static void free_device(pcgpu_mlpc *key) { free_device(&key->key); }
+static void free_device(pcgpu_brakedown *code) { rt::dev_free(code->d_mem); }
+static void free_device(pcgpu_ipa *) {}
+
+// Every creating entry point: *out is cleared whenever out is non-null, then make(handle) fills a fresh handle under the
+// context's lock.  *out receives the handle only when make succeeds; on failure its device memory is freed and it is deleted.
+template <class H, class F>
+static int create(pcgpu_ctx *ctx, bool bad_args, H **out, F make) {
+  if (out) *out = nullptr;
+  return on_ctx(ctx, bad_args || !out, [&]() -> int {
+    H *h = new (std::nothrow) H();
+    if (!h) return PCGPU_E_OOM;
+    int rc = make(h);
+    if (rc) { free_device(h); delete h; return rc; }
+    *out = h;
+    return PCGPU_OK;
+  });
 }
 
-static void brakedown_free(pcgpu_brakedown *code) { rt::dev_free(code->d_mem); }
-
-// frees device memory that work queued on the context may still read: waits for its stream first (no context: frees at once)
-template <class F>
-static void release_after_stream(pcgpu_ctx *ctx, F free_buffers) {
-  if (!ctx) { free_buffers(); return; }
-  std::lock_guard<std::mutex> lk(ctx->mu);
+// Frees a handle whose device memory work queued on the context may still read: waits for its stream first (no context:
+// frees at once).
+template <class H>
+static void release_after_stream(pcgpu_ctx *ctx, H *h) {
+  if (!h) return;
+  std::unique_lock<std::mutex> lk;
+  if (ctx) {
+    lk = std::unique_lock<std::mutex>(ctx->mu);
 #ifndef PCGPU_EMUL
-  cudaSetDevice(ctx->device);
-  cudaStreamSynchronize(ctx->stream);
+    cudaSetDevice(ctx->device);
+    cudaStreamSynchronize(ctx->stream);
 #endif
-  free_buffers();
+  }
+  free_device(h);
+  delete h;
 }
 
 PCGPU_INSTANTIATE(Bls12381, extern)
@@ -155,24 +175,13 @@ extern "C" int pcgpu_profile_get(pcgpu_ctx *ctx, int stage, double *ms, uint64_t
 
 extern "C" int pcgpu_srs_register(pcgpu_ctx *ctx, int curve, const void *bases_xy, const uint8_t *inf, size_t n,
                                   uint32_t flags, pcgpu_srs **out) {
-  const bool bad_args = !out || (n && !bases_xy) || n >= (1u << 26);
-  if (ctx && !bad_args) *out = nullptr;
-  return on_ctx(ctx, bad_args, [&]() -> int {
-    pcgpu_srs *srs = new (std::nothrow) pcgpu_srs();
-    if (!srs) return PCGPU_E_OOM;
-    srs->curve = curve; srs->n = n; srs->d_tables = nullptr; srs->d_folded = nullptr; srs->c = 0; srs->groups = 1; srs->d_comb = nullptr; srs->comb_c = 0;
-    int rc = [&]() -> int { DISPATCH_GROUP(curve, return srs_register_impl<C>(ctx, bases_xy, inf, n, flags, srs)); }();
-    if (rc) { srs_free(srs); delete srs; return rc; }
-    *out = srs;
-    return PCGPU_OK;
+  return create(ctx, (n && !bases_xy) || n >= (1u << 26), out, [&](pcgpu_srs *srs) -> int {
+    srs->curve = curve; srs->n = n;
+    DISPATCH_GROUP(curve, return srs_register_impl<C>(ctx, bases_xy, inf, n, flags, srs));
   });
 }
 
-extern "C" void pcgpu_srs_release(pcgpu_ctx *ctx, pcgpu_srs *srs) {
-  if (!srs) return;
-  release_after_stream(ctx, [&] { srs_free(srs); });
-  delete srs;
-}
+extern "C" void pcgpu_srs_release(pcgpu_ctx *ctx, pcgpu_srs *srs) { release_after_stream(ctx, srs); }
 
 extern "C" size_t pcgpu_srs_len(const pcgpu_srs *srs) { return srs ? srs->n : 0; }
 extern "C" int pcgpu_srs_curve(const pcgpu_srs *srs) { return srs ? srs->curve : -1; }
@@ -218,26 +227,14 @@ extern "C" int pcgpu_g2_fixed_base_mul(pcgpu_ctx *ctx, int group, const void *ba
 // ---- MultilinearPC (mlpc.cuh) -------------------------------------------------------------------------------------------
 extern "C" int pcgpu_mlpc_register(pcgpu_ctx *ctx, int curve, uint32_t nv, const void *const *powers_of_h, const uint8_t *const *inf,
                                    uint32_t flags, pcgpu_mlpc **out) {
-  const bool bad_args = !out || !powers_of_h || nv == 0 || nv > 25 || (flags & ~(uint32_t)PCGPU_DEVICE_PTRS);
-  if (ctx && out) *out = nullptr;
-  return on_ctx(ctx, bad_args, [&]() -> int {
-    pcgpu_mlpc *m = new (std::nothrow) pcgpu_mlpc();
-    if (!m) return PCGPU_E_OOM;
+  const bool bad_args = !powers_of_h || nv == 0 || nv > 25 || (flags & ~(uint32_t)PCGPU_DEVICE_PTRS);
+  return create(ctx, bad_args, out, [&](pcgpu_mlpc *m) -> int {
     m->curve = curve; m->nv = nv;
-    m->key.curve = curve == PCGPU_BLS12_381 ? PCGPU_BLS12_381_G2 : PCGPU_BN254_G2;
-    m->key.d_tables = nullptr; m->key.d_folded = nullptr; m->key.d_comb = nullptr; m->key.comb_c = 0;
-    int rc = [&]() -> int { DISPATCH_PAIRING_G2(curve, return mlpc_register_impl<C>(ctx, nv, powers_of_h, inf, flags, m)); }();
-    if (rc) { srs_free(&m->key); delete m; return rc; }
-    *out = m;
-    return PCGPU_OK;
+    DISPATCH_PAIRING_G2(curve, return mlpc_register_impl<C>(ctx, nv, powers_of_h, inf, flags, m));
   });
 }
 
-extern "C" void pcgpu_mlpc_release(pcgpu_ctx *ctx, pcgpu_mlpc *key) {
-  if (!key) return;
-  release_after_stream(ctx, [&] { srs_free(&key->key); });
-  delete key;
-}
+extern "C" void pcgpu_mlpc_release(pcgpu_ctx *ctx, pcgpu_mlpc *key) { release_after_stream(ctx, key); }
 
 extern "C" int pcgpu_mlpc_open(pcgpu_ctx *ctx, const pcgpu_mlpc *key, const void *evals, size_t n, const void *point, uint32_t flags,
                                void *out_proofs_xy, uint8_t *out_proofs_inf, void *out_value) {
@@ -338,22 +335,20 @@ extern "C" int pcgpu_msm_batch(pcgpu_ctx *ctx, const pcgpu_srs *srs, const void 
 
 extern "C" int pcgpu_ipa_begin(pcgpu_ctx *ctx, int curve, const void *comm_key_xy, size_t n, const void *coeffs, size_t n_coeffs,
                                const void *point, uint32_t flags, pcgpu_ipa **out) {
-  const bool bad_args = !out || !comm_key_xy || !point || n == 0 || (n & (n - 1)) || n_coeffs > n || (n_coeffs && !coeffs);
-  if (ctx && !bad_args) *out = nullptr;
-  return on_ctx(ctx, bad_args, [&]() -> int {
-    pcgpu_ipa *st = new (std::nothrow) pcgpu_ipa();
-    if (!st) return PCGPU_E_OOM;
+  const bool bad_args = !comm_key_xy || !point || n == 0 || (n & (n - 1)) || n_coeffs > n || (n_coeffs && !coeffs);
+  return create(ctx, bad_args, out, [&](pcgpu_ipa *st) -> int {
+    if (ctx->ipa_active) return PCGPU_E_BADARG;   // one halving loop at a time per context: the state lives in its IPA arena
     int rc = [&]() -> int { DISPATCH_CURVE(curve, return ipa_begin_impl<C>(ctx, comm_key_xy, n, coeffs, n_coeffs, point, flags, st)); }();
-    if (rc) { if (rc != PCGPU_E_BADARG) ctx->ipa_active = false; delete st; return rc; }
-    *out = st;
-    return PCGPU_OK;
+    if (rc == PCGPU_OK) { st->ctx = ctx; ctx->ipa_active = true; }
+    return rc;
   });
 }
 
+// the IPA calls after begin run only on the context that began the open (pcgpu_ipa::ctx)
 extern "C" int pcgpu_ipa_round_lr(pcgpu_ctx *ctx, pcgpu_ipa *st, const void *h_prime_xy, void *out_l_xy, uint8_t *out_l_inf,
                                   void *out_r_xy, uint8_t *out_r_inf) {
   return guarded([&]() -> int {
-  if (!ctx || !st || !h_prime_xy || !out_l_xy || !out_r_xy) return PCGPU_E_BADARG;
+  if (!ctx || !st || st->ctx != ctx || !h_prime_xy || !out_l_xy || !out_r_xy) return PCGPU_E_BADARG;
   int src = ensure_siblings(ctx, 1);   // the two commitments of a round run on two streams
   if (src) return src;
   pcgpu_ctx *sib = ctx->siblings[0];
@@ -365,7 +360,7 @@ extern "C" int pcgpu_ipa_round_lr(pcgpu_ctx *ctx, pcgpu_ipa *st, const void *h_p
 }
 
 extern "C" int pcgpu_ipa_round_fold(pcgpu_ctx *ctx, pcgpu_ipa *st, const void *challenge, const void *challenge_inv) {
-  return on_ctx(ctx, !st || !challenge || !challenge_inv, [&]() -> int {
+  return on_ctx(ctx, !st || st->ctx != ctx || !challenge || !challenge_inv, [&]() -> int {
     DISPATCH_CURVE(st->curve, return ipa_round_fold_impl<C>(ctx, st, challenge, challenge_inv));
   });
 }
@@ -373,7 +368,7 @@ extern "C" int pcgpu_ipa_round_fold(pcgpu_ctx *ctx, pcgpu_ipa *st, const void *c
 extern "C" size_t pcgpu_ipa_len(const pcgpu_ipa *st) { return st ? st->n : 0; }
 
 extern "C" int pcgpu_ipa_finish(pcgpu_ctx *ctx, pcgpu_ipa *st, void *out_final_key_xy, void *out_c) {
-  return on_ctx(ctx, !st, [&]() -> int {
+  return on_ctx(ctx, !st || st->ctx != ctx, [&]() -> int {
     int rc = [&]() -> int { DISPATCH_CURVE(st->curve, return ipa_finish_impl<C>(ctx, st, out_final_key_xy, out_c)); }();
     ctx->ipa_active = false;   // the state's memory belongs to the context's IPA arena and is kept for the next open
     delete st;
@@ -624,25 +619,12 @@ extern "C" int pcgpu_brakedown_register(pcgpu_ctx *ctx, int curve, size_t m, siz
                                         const uint64_t *b_dims, const uint64_t *const *ind_ptr, const uint64_t *const *col_ind,
                                         const void *const *val, uint32_t flags, pcgpu_brakedown **out) {
   (void)flags;
-  if (ctx && out) *out = nullptr;
-  return on_ctx(ctx, !out, [&]() -> int {
-    pcgpu_brakedown *bd = new (std::nothrow) pcgpu_brakedown();
-    if (!bd) return PCGPU_E_OOM;
-    bd->d_mem = nullptr;
-    int rc = [&]() -> int {
-      DISPATCH_CURVE(curve, return brakedown_register_impl<C>(ctx, m, m_ext, levels, a_dims, b_dims, ind_ptr, col_ind, val, bd));
-    }();
-    if (rc) { brakedown_free(bd); delete bd; return rc; }
-    *out = bd;
-    return PCGPU_OK;
+  return create(ctx, false, out, [&](pcgpu_brakedown *bd) -> int {
+    DISPATCH_CURVE(curve, return brakedown_register_impl<C>(ctx, m, m_ext, levels, a_dims, b_dims, ind_ptr, col_ind, val, bd));
   });
 }
 
-extern "C" void pcgpu_brakedown_release(pcgpu_ctx *ctx, pcgpu_brakedown *code) {
-  if (!code) return;
-  release_after_stream(ctx, [&] { brakedown_free(code); });
-  delete code;
-}
+extern "C" void pcgpu_brakedown_release(pcgpu_ctx *ctx, pcgpu_brakedown *code) { release_after_stream(ctx, code); }
 
 extern "C" int pcgpu_brakedown_encode(pcgpu_ctx *ctx, const pcgpu_brakedown *code, const void *mat, size_t n_rows, size_t n_cols,
                                       uint32_t flags, void *out_ext) {

@@ -67,15 +67,21 @@ struct Prof {
 };
 
 struct pcgpu_srs {
-  int curve;
-  size_t n;          // bases per table group
-  uint32_t c;        // window bits the groups were built for (0: raw bases only)
-  uint32_t groups;   // table groups (1: raw bases)
-  void *d_tables;    // the n raw bases, packed x||y
-  void *d_folded;    // window-folded tables: groups * n records in the aligned layout (PCGPU_SRS_PRECOMPUTE) or null
-  void *d_comb;      // fixed-base comb tables (PCGPU_SRS_COMB) or null
-  uint32_t comb_c;   // comb window bits
+  int curve = 0;
+  size_t n = 0;                // bases per table group
+  uint32_t c = 0;              // window bits the groups were built for (0: raw bases only)
+  uint32_t groups = 1;         // table groups (1: raw bases)
+  void *d_tables = nullptr;    // the n raw bases, packed x||y
+  void *d_folded = nullptr;    // window-folded tables: groups * n records in the aligned layout (PCGPU_SRS_PRECOMPUTE) or null
+  void *d_comb = nullptr;      // fixed-base comb tables (PCGPU_SRS_COMB) or null
+  uint32_t comb_c = 0;         // comb window bits
 };
+
+// a key of raw bases over n points at d_tables that the caller owns; curve: C's group id (include/pcgpu.h: a G2 group is
+// 0x100 + the curve id)
+template <class C> inline pcgpu_srs srs_view(void *d_tables, size_t n) {
+  return pcgpu_srs{C::EXT == 1 ? C::ID : PCGPU_BLS12_381_G2 + C::ID, n, 0, 1, d_tables};
+}
 
 enum { PCGPU_MAX_PLANES = 512 };  // S * c of any geometry msm_geometry produces (W <= 32 windows of <= 22 bits, S <= W)
 
@@ -98,7 +104,7 @@ struct pcgpu_ctx {
   rt::stream_t own_stream, stream;
   rt::Arena msm_arena, stage;
   rt::Arena ipa_arena;             // state of the (one) InnerProductArgPC::open in progress on this context; reused across opens
-  bool ipa_active = false;
+  bool ipa_active = false;         // an open holds ipa_arena: set by pcgpu_ipa_begin, cleared by pcgpu_ipa_finish (api.cu)
   uint32_t pair_tdiv = 1;          // set by the batch entry points while several pipelines are in flight (msm_plan)
   DeviceWords *d_words = nullptr;
   Prof prof;
@@ -111,6 +117,12 @@ struct pcgpu_ctx {
   uint64_t last_geom[PCGPU_GEOM_FIELDS] = {0};   // path / geometry of the most recent MSM (pcgpu_msm_last_geometry)
   std::mutex mu;
 };
+
+// the caller's bulk input into a device buffer that is already allocated: device-to-device under PCGPU_DEVICE_PTRS, else
+// host-to-device
+inline int copy_in(void *dst, const void *src, size_t bytes, uint32_t flags, rt::stream_t s) {
+  return flags & PCGPU_DEVICE_PTRS ? rt::copy_d2d(dst, src, bytes, s) : rt::copy_h2d(dst, src, bytes, s);
+}
 
 #ifndef PCGPU_EMUL
 #define SET_DEVICE(ctx) do { if (cudaSetDevice((ctx)->device) != cudaSuccess) return PCGPU_E_CUDA; } while (0)
@@ -250,9 +262,7 @@ int srs_register_impl(pcgpu_ctx *ctx, const void *bases, const uint8_t *inf, siz
   if (groups > 1 && (rc = rt::dev_malloc(&srs->d_folded, (size_t)aligned_pt_words<C>() * 4 * n * groups))) return rc;
   rt::stream_t st = ctx->stream;
   if (n) {
-    if (flags & PCGPU_DEVICE_PTRS) rc = rt::copy_d2d(srs->d_tables, bases, psz * n, st);
-    else rc = rt::copy_h2d(srs->d_tables, bases, psz * n, st);
-    if (rc) return rc;
+    if ((rc = copy_in(srs->d_tables, bases, psz * n, flags, st))) return rc;
     if (inf) {   // identity bases become the device's (0, 0) encoding -- one kernel, for host and device flag arrays alike
       const uint8_t *d_inf;
       Staging io(ctx, flags);
@@ -668,8 +678,8 @@ int fixed_base_impl(pcgpu_ctx *ctx, const void *base_xy, const void *scalars, si
 // MultilinearPC (mlpc.cuh): committer key with pair-folded G2 bases, open = fold chain + nv G2 MSMs
 // ---------------------------------------------------------------------------------------------
 struct pcgpu_mlpc {
-  int curve;        // the pairing curve (PCGPU_BLS12_381 / PCGPU_BN254)
-  uint32_t nv;
+  int curve = 0;    // the pairing curve (PCGPU_BLS12_381 / PCGPU_BN254)
+  uint32_t nv = 0;
   pcgpu_srs key;    // every level's folded bases, level i at mlpc_level_offset(nv, i); key.curve is the G2 group id
 };
 
@@ -680,7 +690,9 @@ int mlpc_register_impl(pcgpu_ctx *ctx, uint32_t nv, const void *const *powers_of
   rt::stream_t st = ctx->stream;
   int rc;
   for (uint32_t i = 0; i < nv; i++) if (!powers_of_h[i]) return PCGPU_E_BADARG;
-  if ((rc = rt::dev_malloc(&m->key.d_tables, psz * (n0 - 1)))) return rc;
+  void *d_tables;
+  if ((rc = rt::dev_malloc(&d_tables, psz * (n0 - 1)))) return rc;
+  m->key = srs_view<C>(d_tables, n0 - 1);
   Affine<C> *raw; uint8_t *d_inf;
   Staging io(ctx, 0);
   io.scratch(raw, psz * n0);
@@ -688,20 +700,15 @@ int mlpc_register_impl(pcgpu_ctx *ctx, uint32_t nv, const void *const *powers_of
   if ((rc = io.upload())) return rc;
   for (uint32_t i = 0; i < nv; i++) {
     const size_t len = n0 >> i;
-    if (flags & PCGPU_DEVICE_PTRS) rc = rt::copy_d2d(raw, powers_of_h[i], psz * len, st);
-    else rc = rt::copy_h2d(raw, powers_of_h[i], psz * len, st);
-    if (rc) return rc;
+    if ((rc = copy_in(raw, powers_of_h[i], psz * len, flags, st))) return rc;
     if (inf && inf[i]) {
-      if (flags & PCGPU_DEVICE_PTRS) rc = rt::copy_d2d(d_inf, inf[i], len, st);
-      else rc = rt::copy_h2d(d_inf, inf[i], len, st);
-      if (rc) return rc;
+      if ((rc = copy_in(d_inf, inf[i], len, flags, st))) return rc;
       if ((rc = rt::launch<256>(SrsZeroIdentityBody{(uint32_t *)raw, d_inf, (uint32_t)(psz / 4)}, len, st))) return rc;
     }
     Affine<C> *out = (Affine<C> *)m->key.d_tables + mlpc_level_offset(nv, i);
     if ((rc = rt::launch<128>(PairFoldBasesBody<C>{raw, out}, len / 2, st))) return rc;
     if ((rc = rt::stream_sync(st))) return rc;   // the next level's upload overwrites raw
   }
-  m->key.n = n0 - 1; m->key.c = 0; m->key.groups = 1;
   return PCGPU_OK;
 }
 
@@ -1035,17 +1042,18 @@ int kzg_commit_open_impl(pcgpu_ctx *ctx, pcgpu_ctx *sib, const pcgpu_srs *pg, co
 // ---------------------------------------------------------------------------------------------
 // Device buffers are carved from the context's IPA arena by ipa_begin.
 struct pcgpu_ipa {
-  int curve; size_t n0, n;
-  void *d_key;               // n0 affine points (folded in place until the key is frozen)
-  uint32_t *d_coeffs, *d_z;  // n0 Fr each
-  uint32_t *d_ip_scratch;    // fr_inner_product's scratch
-  uint32_t *d_point;         // the evaluation point z (1 Fr)
-  uint32_t *d_ip;            // <coeffs_r, z_l>, <coeffs_l, z_r> (2 Fr)
-  uint32_t *d_ch, *d_chi;    // the round's challenge and its inverse (1 Fr each)
-  void *d_h;                 // h' (one affine point)
+  pcgpu_ctx *ctx = nullptr;  // the context that began the open: the only one whose arena and pow2 tables it may use
+  int curve = 0; size_t n0 = 0, n = 0;
+  void *d_key = nullptr;     // n0 affine points (folded in place until the key is frozen)
+  uint32_t *d_coeffs = nullptr, *d_z = nullptr;   // n0 Fr each
+  uint32_t *d_ip_scratch = nullptr;   // fr_inner_product's scratch
+  uint32_t *d_point = nullptr;        // the evaluation point z (1 Fr)
+  uint32_t *d_ip = nullptr;           // <coeffs_r, z_l>, <coeffs_l, z_r> (2 Fr)
+  uint32_t *d_ch = nullptr, *d_chi = nullptr;   // the round's challenge and its inverse (1 Fr each)
+  void *d_h = nullptr;       // h' (one affine point)
   pcgpu_srs view;            // non-owning SRS view over d_key for the MSM pipeline
-  size_t frozen_m;           // 0: the key is folded explicitly; else the key stays at frozen_m points (ipa.cuh, "late rounds")
-  uint32_t *d_w, *d_sl, *d_sr;   // frozen key: the weights and the l / r MSM scalars (SMALL_MAX_N Fr each)
+  size_t frozen_m = 0;       // 0: the key is folded explicitly; else the key stays at frozen_m points (ipa.cuh, "late rounds")
+  uint32_t *d_w = nullptr, *d_sl = nullptr, *d_sr = nullptr;   // frozen key: the weights and the l / r MSM scalars (SMALL_MAX_N Fr each)
 };
 
 template <class C>
@@ -1075,11 +1083,9 @@ int ipa_begin_impl(pcgpu_ctx *ctx, const void *key_xy, size_t n, const void *coe
   using R = typename C::Fr;
   rt::stream_t s = ctx->stream;
   int rc;
-  bool dev = (flags & PCGPU_DEVICE_PTRS) != 0;
-  st->curve = C::ID; st->n0 = st->n = n; st->frozen_m = 0;
+  st->curve = C::ID; st->n0 = st->n = n;
   if ((rc = ensure_pow2<C>(ctx))) return rc;
   // one arena per context, grown on demand and kept: an open costs no cudaMalloc / cudaFree after the first
-  if (ctx->ipa_active) return PCGPU_E_BADARG;          // one halving loop at a time per context
   Affine<C> *key, *h;
   rc = ctx->ipa_arena.carve([&](auto &&buf) {
     buf(key, n); buf(st->d_coeffs, 8 * n); buf(st->d_z, 8 * n); buf(st->d_ip_scratch, 8 * (IP_THREADS + IP_THREADS / IP_BLOCK));
@@ -1088,14 +1094,12 @@ int ipa_begin_impl(pcgpu_ctx *ctx, const void *key_xy, size_t n, const void *coe
   });
   if (rc) return rc;
   st->d_key = key; st->d_h = h;
-  ctx->ipa_active = true;
-  if ((rc = dev ? rt::copy_d2d(st->d_key, key_xy, n * sizeof(Affine<C>), s) : rt::copy_h2d(st->d_key, key_xy, n * sizeof(Affine<C>), s))) return rc;
+  if ((rc = copy_in(st->d_key, key_xy, n * sizeof(Affine<C>), flags, s))) return rc;
   if ((rc = rt::dev_memset(st->d_coeffs, 0, n * 32, s))) return rc;
-  if (n_coeffs && (rc = dev ? rt::copy_d2d(st->d_coeffs, coeffs, n_coeffs * 32, s) : rt::copy_h2d(st->d_coeffs, coeffs, n_coeffs * 32, s))) return rc;
+  if (n_coeffs && (rc = copy_in(st->d_coeffs, coeffs, n_coeffs * 32, flags, s))) return rc;
   if ((rc = rt::copy_h2d(st->d_point, point, 32, s))) return rc;
   if ((rc = rt::launch<128>(FrPowersBody<R>{st->d_point, st->d_z}, n, s))) return rc;
-  st->view.curve = C::ID; st->view.n = n; st->view.c = 0; st->view.groups = 1; st->view.d_tables = st->d_key; st->view.d_folded = nullptr;
-  st->view.d_comb = nullptr; st->view.comb_c = 0;
+  st->view = srs_view<C>(st->d_key, n);
   if ((rc = ipa_maybe_freeze<C>(ctx, st))) return rc;
   return rt::stream_sync(s);
 }
@@ -1429,11 +1433,11 @@ int lincode_commit_impl(pcgpu_ctx *ctx, const void *mat, size_t n_rows, size_t n
 // BrakedownPCParams' code (linear_codes/brakedown.rs:146-203) on the device.  start / end as brakedown.rs:168-181; the
 // Reed-Solomon bounds as multilinear_brakedown/mod.rs:71-73 (with the unwrap_or defaults when there are no levels).
 struct pcgpu_brakedown {
-  int curve;
-  uint64_t m, m_ext, levels;
+  int curve = 0;
+  uint64_t m = 0, m_ext = 0, levels = 0;
   std::vector<uint64_t> a_dims, b_dims, start, end;   // 3L, 3L, L, L
-  uint64_t rss, rsie, rsoe;
-  uint32_t *d_mem;                                    // every matrix: ind_ptr | col_ind | val, one allocation
+  uint64_t rss = 0, rsie = 0, rsoe = 0;
+  uint32_t *d_mem = nullptr;                          // every matrix: ind_ptr | col_ind | val, one allocation
   std::vector<SprsLevel> a_lev, b_lev;
 };
 
