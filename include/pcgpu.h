@@ -76,7 +76,8 @@ int pcgpu_set_stream(pcgpu_ctx *ctx, void *cuda_stream);
 /* Per-stage device timings (CUDA events on the launching stream).  stage: 0 digits/count, 1 scan,
  * 2 scatter, 3 tasks, 4 bucket accumulate (XYZZ), 5 bucket reduce, 6 final (host tail, wall clock), 7 fr division,
  * 8 fr axpy, 9 ntt, 10 comb batch, 11 affine pair rounds (all), 12 affine pair round 0 kernel alone, 13 peer push + wait,
- * 14 column hashes + Merkle tree, 15 Brakedown encoding, 16 MultilinearPC open fold chain.
+ * 14 column hashes + Merkle tree, 15 Brakedown encoding, 16 MultilinearPC open fold chain, 17 pairing Miller loops + final
+ * exponentiations.
  * enable=1 starts recording; get returns accumulated milliseconds and launch count since enable. */
 int pcgpu_profile_enable(pcgpu_ctx *ctx, int enable);
 int pcgpu_profile_get(pcgpu_ctx *ctx, int stage, double *ms, uint64_t *count);
@@ -338,6 +339,25 @@ void pcgpu_mlpc_release(pcgpu_ctx *ctx, pcgpu_mlpc *key);
 int pcgpu_mlpc_open(pcgpu_ctx *ctx, const pcgpu_mlpc *key, const void *evals, size_t n, const void *point, uint32_t flags,
                     void *out_proofs_xy, uint8_t *out_proofs_inf, void *out_value);
 
+/* ---- pairing (verifiers) ----------------------------------------------------------------------------------------------
+ * E::multi_pairing(a, b) for `count` independent equations of k pairs each: equation j is
+ * prod_{i<k} e(P[j*k+i], Q[j*k+i]) (kzg10/mod.rs:326-330, :382-387; multilinear_pc/mod.rs:179-199; sonic_pc/mod.rs:128), the
+ * optimal-ate pairing with the exact final exponentiation (p^12 - 1) / r.  curve: PCGPU_BLS12_381 or PCGPU_BN254 (any other
+ * id, G2 ids included: PCGPU_E_BADARG).
+ *   g1_xy: count * k G1 affine points (x || y); g2_xy: count * k G2 affine points (x.c0 x.c1 y.c0 y.c1); g1_inf / g2_inf: their
+ *   identity bytes, either may be NULL.  A pair with an identity on either side contributes 1.  With PCGPU_DEVICE_PTRS the
+ *   four input arrays are device pointers; the outputs are host arrays.
+ *   out_gt: count Fq12 elements, 12 Fq coefficients each in ark's order (c0.c0.c0, c0.c0.c1, c0.c1.c0 ... c1.c2.c1), each
+ *   `limbs` u64 Montgomery (tower Fq6 = Fq2[v]/(v^3 - xi), Fq12 = Fq6[w]/(w^2 - v), xi = 1 + u on BLS12-381, 9 + u on
+ *   BN254); out_is_one: count bytes, 1 where the equation's product is one.  Either output may be NULL, not both.
+ *   k == 0 gives the identity (ark's empty multi_pairing); k > PCGPU_PAIRING_MAX_K: PCGPU_E_BADARG; count == 0 is a no-op.
+ * Points are NOT validated (on the curve, in the subgroup), as G1Prepared::from / G2Prepared::from do not validate either:
+ * pass points decoded with validation.  Profile stage 17.  One equation is a serial chain in one thread; the device pays off
+ * with many equations per call. */
+#define PCGPU_PAIRING_MAX_K 64
+int pcgpu_multi_pairing(pcgpu_ctx *ctx, int curve, const void *g1_xy, const uint8_t *g1_inf, const void *g2_xy,
+                        const uint8_t *g2_inf, size_t k, size_t count, uint32_t flags, void *out_gt, uint8_t *out_is_one);
+
 /* ---- KZG10 fused prover calls ------------------------------------------------------------------ */
 /* KZG10::commit -- kzg10/mod.rs:157-210.  coeffs: n Montgomery Fr (low degree first; trailing zeros allowed and
  * ignored like DensePolynomial's truncation).  Hiding: pass gamma (powers_of_gamma_g) and n_blind > 0 blinding
@@ -415,10 +435,12 @@ enum { PCGPU_MSM_PATH_NONE = 0, PCGPU_MSM_PATH_SMALL = 1, PCGPU_MSM_PATH_BUCKETS
 int pcgpu_msm_last_geometry(pcgpu_ctx *ctx, uint64_t *out, size_t len);
 /* One field primitive applied elementwise on the device (the same code the kernels use), for testing the field layer
  * against plain integers: which = 0 the base field Fq of `curve`, 1 its scalar field Fr, 2 its quadratic extension Fq2
- * (pairing curves only; elements c0 || c1; ops 0, 2, 3, 4, 5 (through the norm) and 9 (a^2)).  a, b, out: host arrays of n
+ * (pairing curves only; elements c0 || c1; ops 0, 2, 3, 4, 5 (through the norm) and 9 (a^2)), 3 the pairing's Fq12 (pairing
+ * curves only; elements in pcgpu_multi_pairing's GT layout; ops 0, 2, 3, 4, 5, 9, 10 and 11).  a, b, out: host arrays of n
  * elements, little-endian 32-bit limbs (Fq of BLS12-381: 12 limbs, every other field 8), Montgomery form.  op:
  *   0 mont_mul(a, b)   1 mont_mul_ref(a, b) (plain 64-bit accumulate)   2 a + b   3 a - b   4 -a   5 a^-1 (Fermat)
  *   6 mont_mul2(a, b, b, -a) (= 0)   7 mont_mul2(a, b, a + b, b - a)   8 a^-1 (binary GCD)   9 mont_sqr(a)
+ *   10 a^p (Frobenius, Fq12 only)   11 a^((p^12 - 1) / r) (the final exponentiation, Fq12 only)
  * Ops 6 and 7 fall back to two products on a field without mont_mul2; inverses of 0 are 0. */
 int pcgpu_diag_field_op(pcgpu_ctx *ctx, int curve, int which, int op, const void *a, const void *b, void *out, size_t n);
 

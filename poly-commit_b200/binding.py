@@ -101,6 +101,7 @@ def _load(path):
         "pcgpu_selftest_field": [_vp, ctypes.c_int, ctypes.c_uint64, _sz, ctypes.POINTER(ctypes.c_uint64)],
         "pcgpu_msm_last_geometry": [_vp, ctypes.POINTER(ctypes.c_uint64), _sz],
         "pcgpu_diag_field_op": [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp, _sz],
+        "pcgpu_multi_pairing": [_vp, ctypes.c_int, _vp, _vp, _vp, _vp, _sz, _sz, ctypes.c_uint32, _vp, _vp],
         "pcgpu_ipa_begin": [_vp, ctypes.c_int, _vp, _sz, _vp, _sz, _vp, ctypes.c_uint32, ctypes.POINTER(_vp)],
         "pcgpu_ipa_round_lr": [_vp, _vp, _vp, _vp, _vp, _vp, _vp],
         "pcgpu_ipa_round_fold": [_vp, _vp, _vp, _vp],
@@ -341,15 +342,32 @@ class Engine:
         return g
 
     def diag_field_op(self, curve, which, op, a, b):
-        """one field primitive elementwise on the device (pcgpu_diag_field_op): which 0 = Fq, 1 = Fr, 2 = Fq2 of `curve`; a, b:
-        (n, limbs) uint64 Montgomery elements (limbs = 6 for BLS12-381 Fq, else 4; twice that for Fq2, c0 then c1); returns the
-        (n, limbs) results."""
+        """one field primitive elementwise on the device (pcgpu_diag_field_op): which 0 = Fq, 1 = Fr, 2 = Fq2, 3 = Fq12 of
+        `curve`; a, b: (n, limbs) uint64 Montgomery elements (limbs = 6 for BLS12-381 Fq, else 4; twice that for Fq2, c0 then
+        c1; twelve times that for Fq12, in multi_pairing's GT layout); returns the (n, limbs) results."""
         a, b = _u64(a), _u64(b)
         if a.shape != b.shape:
             raise ValueError("operand shapes differ")
         out = np.zeros_like(a)
         self._ck(self.lib.pcgpu_diag_field_op(self.ctx, curve, which, op, _ptr(a), _ptr(b), _ptr(out), a.shape[0]))
         return out
+
+    # ---- pairing ----
+    def multi_pairing(self, curve, g1, g2, k, g1_inf=None, g2_inf=None, flags=0, count=None):
+        """E::multi_pairing for count equations of k pairs each (pcgpu_multi_pairing).  g1: (count * k, 2*limbs) G1 affine
+        points, g2: (count * k, 4*limbs) G2 affine points, g1_inf / g2_inf: None or identity bytes; with DEVICE_PTRS all four are
+        device pointers and count must be given (else it is len(g1) / k, and 1 for k = 0).  Returns (gt (count, 12*limbs) uint64
+        Montgomery Fq12 in the tower layout, is_one (count,) uint8)."""
+        g1, g2 = _u64(g1), _u64(g2)
+        if count is None:
+            count = (g1.size // (2 * fq_limbs(curve))) // k if k else 1
+        g1_inf, g2_inf = (f if f is None or isinstance(f, (int, np.integer)) else np.ascontiguousarray(f, dtype=np.uint8)
+                          for f in (g1_inf, g2_inf))
+        gt = np.zeros((count, 12 * fq_limbs(curve)), dtype=np.uint64)
+        one = np.zeros(count, dtype=np.uint8)
+        self._ck(self.lib.pcgpu_multi_pairing(self.ctx, curve, _ptr(g1), _ptr(g1_inf), _ptr(g2), _ptr(g2_inf), k, count, flags,
+                                              _ptr(gt), _ptr(one)))
+        return gt, one
 
     # ---- SRS ----
     def srs_register(self, curve, bases_xy, inf=None, n=None, flags=0):

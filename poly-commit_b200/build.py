@@ -16,8 +16,9 @@ CURVES = ["Bls12381", "Bn254", "Pallas"]
 GROUPS = [6, 8, 9, 5, 2, 3, 1, 4]   # inst_unit.cu groups, heaviest first (see the list at the top of that file)
 PAIRING_CURVES = ["Bls12381", "Bn254"]
 G2_GROUPS = [11, 12, 10]           # G2 point kernels and entry points: the pairing curves only
+PAIRING_GROUPS = [13]              # Miller loops and final exponentiations: the pairing curves only
 # heaviest first so the thread pool keeps every core busy to the end
-UNITS = [("inst_unit", c, g) for g in G2_GROUPS[:1] for c in PAIRING_CURVES] + \
+UNITS = [("inst_unit", c, g) for g in PAIRING_GROUPS + G2_GROUPS[:1] for c in PAIRING_CURVES] + \
     [("inst_unit", c, g) for g in GROUPS for c in CURVES] + \
     [("inst_unit", c, g) for g in G2_GROUPS[1:] for c in PAIRING_CURVES] + [("api", None, None)]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]

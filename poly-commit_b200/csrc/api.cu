@@ -72,6 +72,8 @@ PCGPU_INSTANTIATE(Bn254, extern)
 PCGPU_INSTANTIATE(Pallas, extern)
 PCGPU_INSTANTIATE_G2(Bls12381G2, extern)
 PCGPU_INSTANTIATE_G2(Bn254G2, extern)
+PCGPU_INST_PAIRING(Bls12381, extern)
+PCGPU_INST_PAIRING(Bn254, extern)
 
 extern "C" const char *pcgpu_strerror(int code) {
   switch (code) {
@@ -243,6 +245,16 @@ extern "C" int pcgpu_mlpc_open(pcgpu_ctx *ctx, const pcgpu_mlpc *key, const void
   });
 }
 
+// ---- pairing (pairing.cuh) ----------------------------------------------------------------------------------------------
+extern "C" int pcgpu_multi_pairing(pcgpu_ctx *ctx, int curve, const void *g1_xy, const uint8_t *g1_inf, const void *g2_xy,
+                                   const uint8_t *g2_inf, size_t k, size_t count, uint32_t flags, void *out_gt, uint8_t *out_is_one) {
+  const bool bad_args = k > PCGPU_PAIRING_MAX_K || (!out_gt && !out_is_one) || (k && count && (!g1_xy || !g2_xy)) ||
+                        (flags & ~(uint32_t)PCGPU_DEVICE_PTRS);
+  return on_ctx(ctx, bad_args, [&]() -> int {
+    DISPATCH_PAIRING(curve, return multi_pairing_impl<C>(ctx, g1_xy, g1_inf, g2_xy, g2_inf, k, count, flags, out_gt, out_is_one));
+  });
+}
+
 extern "C" int pcgpu_fr_from_mont(pcgpu_ctx *ctx, int curve, const void *in, void *out, size_t n, uint32_t flags) {
   return on_ctx(ctx, (n && (!in || !out)), [&]() -> int {
     DISPATCH_CURVE(curve, return fr_from_mont_impl<C>(ctx, in, out, n, flags));
@@ -312,8 +324,9 @@ extern "C" int pcgpu_msm_last_geometry(pcgpu_ctx *ctx, uint64_t *out, size_t len
 }
 
 extern "C" int pcgpu_diag_field_op(pcgpu_ctx *ctx, int curve, int which, int op, const void *a, const void *b, void *out, size_t n) {
-  return on_ctx(ctx, which < 0 || which > 2 || op < 0 || op > 9 || (n && (!a || !b || !out)), [&]() -> int {
+  return on_ctx(ctx, which < 0 || which > 3 || op < 0 || op > (which == 3 ? 11 : 9) || (n && (!a || !b || !out)), [&]() -> int {
     if (which == 2) { DISPATCH_PAIRING_G2(curve, return diag_fq2_op_impl<C>(ctx, op, a, b, out, n)); }
+    if (which == 3) { DISPATCH_PAIRING(curve, return diag_fq12_op_impl<C>(ctx, op, a, b, out, n)); }
     DISPATCH_CURVE(curve, return diag_field_op_impl<C>(ctx, which, op, a, b, out, n));
   });
 }

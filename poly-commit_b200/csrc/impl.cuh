@@ -28,13 +28,14 @@
 #include "sprs.cuh"
 #include "field_ops.cuh"
 #include "mlpc.cuh"
+#include "pairing.cuh"
 
 using namespace pcgpu;
 
 // ---------------------------------------------------------------------------------------------
 // profiling (CUDA events on the launching stream)
 // ---------------------------------------------------------------------------------------------
-enum { PROF_STAGES = 17 };
+enum { PROF_STAGES = 18 };
 struct Prof {
   bool on = false;
   double ms[PROF_STAGES] = {0};
@@ -157,9 +158,18 @@ inline int copy_in(void *dst, const void *src, size_t bytes, uint32_t flags, rt:
     default: return PCGPU_E_BADARG;                      \
   }
 
+// the G1 group of a pairing curve id (pcgpu_multi_pairing, pcgpu_diag_field_op which = 3)
+#define DISPATCH_PAIRING(curve, CALL)                    \
+  switch (curve) {                                       \
+    case PCGPU_BLS12_381: { using C = Bls12381; CALL; }  \
+    case PCGPU_BN254: { using C = Bn254; CALL; }         \
+    default: return PCGPU_E_BADARG;                      \
+  }
+
 // The operands of one call that pass through the context's staging arena.  Each operand is declared once, by what it is:
 //   in       with PCGPU_DEVICE_PTRS the caller's pointer as is, else an arena buffer filled from the host
 //   host_in  always a host pointer: an arena buffer filled from it
+//   host_out always a host pointer (or null): an arena buffer, copied back when the destination is non-null
 //   out      with PCGPU_DEVICE_PTRS and a non-null destination the caller's pointer, else an arena buffer, copied back when
 //            the flag is clear and the destination is non-null
 //   inout    in and out over one buffer
@@ -174,6 +184,7 @@ class Staging {
   template <class P> void in(P &d, const void *src, size_t bytes) { add(d, dev_, src, nullptr, bytes, TO_DEV); }
   template <class P> void host_in(P &d, const void *src, size_t bytes) { add(d, false, src, nullptr, bytes, TO_DEV); }
   template <class P> void out(P &d, void *dst, size_t bytes) { add(d, dev_ && dst, dst, dev_ ? nullptr : dst, bytes, TO_HOST); }
+  template <class P> void host_out(P &d, void *dst, size_t bytes) { add(d, false, nullptr, dst, bytes, TO_HOST); }
   template <class P> void inout(P &d, void *buf, size_t bytes) { add(d, dev_, buf, buf, bytes, TO_DEV | TO_HOST); }
   template <class P> void scratch(P &d, size_t bytes) { add(d, false, nullptr, nullptr, bytes, 0); }
   int upload();
@@ -1811,6 +1822,57 @@ int diag_fq2_op_impl(pcgpu_ctx *ctx, int op, const void *a, const void *b, void 
   return rt::stream_sync(st);
 }
 
+// which = 3: Fq12 of a pairing curve (C is its G1 group)
+template <class C>
+int diag_fq12_op_impl(pcgpu_ctx *ctx, int op, const void *a, const void *b, void *out, size_t n) {
+  using P = typename C::Fq;
+  if (op != 0 && op != 2 && op != 3 && op != 4 && op != 5 && op != 9 && op != 10 && op != 11) return PCGPU_E_BADARG;
+  if (n == 0) return PCGPU_OK;
+  rt::stream_t st = ctx->stream;
+  const size_t bytes = n * Fq12<P>::WORDS * 4;
+  int rc;
+  const uint32_t *da, *db; uint32_t *dout;
+  Staging io(ctx, 0);
+  io.host_in(da, a, bytes);
+  io.host_in(db, b, bytes);
+  io.out(dout, out, bytes);
+  if ((rc = io.upload())) return rc;
+  if ((rc = rt::launch<64>(Fq12OpBody<P>{da, db, dout, op}, n, st))) return rc;
+  if ((rc = io.download())) return rc;
+  return rt::stream_sync(st);
+}
+
+// pcgpu_multi_pairing: the per-pair Miller values live in the staging arena, one kernel computes them (one thread per pair),
+// a second multiplies each equation's k values and runs its final exponentiation (one thread per equation)
+template <class C>
+int multi_pairing_impl(pcgpu_ctx *ctx, const void *g1_xy, const uint8_t *g1_inf, const void *g2_xy, const uint8_t *g2_inf, size_t k,
+                       size_t count, uint32_t flags, void *out_gt, uint8_t *out_is_one) {
+  using P = typename C::Fq;
+  if (count == 0) return PCGPU_OK;
+  rt::stream_t st = ctx->stream;
+  const size_t pairs = k * count;
+  int rc;
+  const uint32_t *d_g1 = nullptr, *d_g2 = nullptr;
+  const uint8_t *d_g1_inf = nullptr, *d_g2_inf = nullptr;
+  uint32_t *d_miller, *d_gt;
+  uint8_t *d_one;
+  Staging io(ctx, flags);
+  io.in(d_g1, g1_xy, pairs * 2 * P::N * 4);
+  io.in(d_g2, g2_xy, pairs * 4 * P::N * 4);
+  if (g1_inf) io.in(d_g1_inf, g1_inf, pairs);
+  if (g2_inf) io.in(d_g2_inf, g2_inf, pairs);
+  io.scratch(d_miller, pairs * Fq12<P>::WORDS * 4);
+  io.host_out(d_gt, out_gt, count * Fq12<P>::WORDS * 4);
+  io.host_out(d_one, out_is_one, count);
+  if ((rc = io.upload())) return rc;
+  ctx->prof.begin(17, st);
+  if ((rc = rt::launch<64>(MillerBody<P>{d_g1, d_g1_inf, d_g2, d_g2_inf, d_miller}, pairs, st))) return rc;
+  if ((rc = rt::launch<64>(FinalExpBody<P>{d_miller, k, d_gt, d_one}, count, st))) return rc;
+  ctx->prof.end(17, st);
+  if ((rc = io.download())) return rc;
+  return rt::stream_sync(st);
+}
+
 template <class C>
 int diag_field_op_impl(pcgpu_ctx *ctx, int which, int op, const void *a, const void *b, void *out, size_t n) {
   if (n == 0) return PCGPU_OK;
@@ -1960,6 +2022,11 @@ inline int measure_imad_peak_impl(pcgpu_ctx *ctx, double *ops_per_s) {
   EXT template int diag_fq2_op_impl<C>(pcgpu_ctx *, int, const void *, const void *, void *, size_t);                      \
   EXT template int mlpc_register_impl<C>(pcgpu_ctx *, uint32_t, const void *const *, const uint8_t *const *, uint32_t, pcgpu_mlpc *); \
   EXT template int mlpc_open_impl<C>(pcgpu_ctx *, const pcgpu_mlpc *, const void *, size_t, const void *, uint32_t, void *, uint8_t *, void *);
+// the pairing (inst_unit.cu group 13, pairing curves only; C is the G1 group)
+#define PCGPU_INST_PAIRING(C, EXT)                                                                                         \
+  EXT template int multi_pairing_impl<C>(pcgpu_ctx *, const void *, const uint8_t *, const void *, const uint8_t *, size_t, size_t, \
+                                         uint32_t, void *, uint8_t *);                                                     \
+  EXT template int diag_fq12_op_impl<C>(pcgpu_ctx *, int, const void *, const void *, void *, size_t);
 #define PCGPU_INSTANTIATE_G2(C, EXT) \
   PCGPU_INST_ACC(C, EXT) PCGPU_INST_REDUCE(C, EXT) PCGPU_INST_PIPE(C, EXT) PCGPU_INST_SMALL(C, EXT) PCGPU_INST_G2(C, EXT)
 #define PCGPU_INSTANTIATE(C, EXT) \

@@ -4,10 +4,11 @@
 //   5 IPA + wire   6 pair-round kernels   8 XYZZ accumulate   9 bucket reduction
 //   G2 of the pairing curves (BLS12-381, BN254) only: 10 pipeline host logic, small MSM, G2 / MultilinearPC entry points
 //   11 G2 XYZZ accumulate   12 G2 bucket reduction
+//   the pairing curves only: 13 the pairing (Miller loops, final exponentiations, Fq12 diagnostics)
 #include "impl.cuh"
 
 #ifndef PCGPU_UNIT_CURVE
-#error "compile with -DPCGPU_UNIT_CURVE=<Bls12381|Bn254|Pallas> -DPCGPU_UNIT_GROUP=<0..9>"
+#error "compile with -DPCGPU_UNIT_CURVE=<Bls12381|Bn254|Pallas> -DPCGPU_UNIT_GROUP=<0..13>"
 #endif
 #define PCGPU_UC PCGPU_UNIT_CURVE
 #define PCGPU_DEF_OR_EXTERN(GROUP, MACRO) PCGPU_DEF_OR_EXTERN_##GROUP(MACRO)
@@ -21,7 +22,13 @@
 PCGPU_INSTANTIATE(PCGPU_UC, )
 #if PCGPU_CAT(PCGPU_PAIRING_, PCGPU_UNIT_CURVE)
 PCGPU_INSTANTIATE_G2(PCGPU_UG2, )
+PCGPU_INST_PAIRING(PCGPU_UC, )
 #endif
+#elif PCGPU_UNIT_GROUP == 13
+#if !PCGPU_CAT(PCGPU_PAIRING_, PCGPU_UNIT_CURVE)
+#error "group 13 (the pairing) exists for the pairing curves only"
+#endif
+PCGPU_INST_PAIRING(PCGPU_UC, )
 #elif PCGPU_UNIT_GROUP >= 10
 #if !PCGPU_CAT(PCGPU_PAIRING_, PCGPU_UNIT_CURVE)
 #error "groups 10-12 (G2) exist for the pairing curves only"

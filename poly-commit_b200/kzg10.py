@@ -1,18 +1,21 @@
-"""Host mirror of the G1 side of KZG10's verifier (poly-commit/src/kzg10/mod.rs) over the C ABI -- SURVEY.md section 8f
-rank 2 ("verifier-side combination MSMs").  Pairings stay with the caller (out of scope, SURVEY section 2): these functions
-return exactly the G1 points the reference feeds to `E::pairing` / `E::multi_pairing`.
+"""Host mirror of KZG10's verifier (poly-commit/src/kzg10/mod.rs) over the C ABI: the G1 combinations on the device MSMs
+(SURVEY.md section 8f rank 2, "verifier-side combination MSMs") and the pairings on pcgpu_multi_pairing.
 
-  check         kzg10/mod.rs:314-333   inner = comm - g * value - gamma_g * random_v          (:322-325)
-  batch_check   kzg10/mod.rs:337-391   total_c = sum r_i (c_i + z_i w_i) - g * sum r_i v_i - gamma_g * sum r_i rv_i,
-                                        total_w = sum r_i w_i                                  (:345-373)
-                                        returns normalize_batch([-total_w, total_c])           (:376-377)
+  check_inner          kzg10/mod.rs:322-325   inner = comm - g * value - gamma_g * random_v
+  check                kzg10/mod.rs:314-333   e(inner, h) == e(w, beta_h - point * h), as one equation
+                                              e(inner, h) * e(-w, beta_h - point * h) == 1
+  batch_check_combine  kzg10/mod.rs:345-377   total_c = sum r_i (c_i + z_i w_i) - g * sum r_i v_i - gamma_g * sum r_i rv_i,
+                                              total_w = sum r_i w_i; returns normalize_batch([-total_w, total_c])
+  batch_check          kzg10/mod.rs:337-391   e(-total_w, beta_h) * e(total_c, h) == 1                  (:382-387)
+
+A verifier key is a dict with the G1 points g, gamma_g and the G2 points h, beta_h (VerifierKey, data_structures.rs:204-220).
 
 The randomizers (u128::rand(rng), :371, the first one fixed to 1, :352) are an argument: they are data to the kernels.
 All field elements are (.., 4) uint64 Montgomery Fr; points are Montgomery x||y rows.
 """
 import numpy as np
 
-from .binding import SCALARS_MONT, fq_limbs
+from .binding import G2_OF, SCALARS_MONT, fq_limbs
 
 from .params import FQ_MODULUS, FR_MODULUS
 
@@ -67,3 +70,47 @@ def batch_check_combine(eng, curve, g, gamma_g, commitments, points, values, pro
     total_w = eng.msm_bases(curve, proofs_w, rnd, flags=SCALARS_MONT)                                        # (:369)
     neg_w = (np.zeros_like(total_w[0]), True) if total_w[1] else (neg_point(curve, total_w[0]), False)
     return neg_w, total_c
+
+
+def _point(pt):
+    """(xy, is_identity) or a bare xy row -> (xy, is_identity)"""
+    if isinstance(pt, tuple):
+        return np.asarray(pt[0], dtype=np.uint64).reshape(-1), bool(pt[1])
+    return np.asarray(pt, dtype=np.uint64).reshape(-1), False
+
+
+def _one_mont(curve):
+    r = FR_MODULUS[curve]
+    v = (1 << 256) % r
+    return np.array([(v >> (64 * j)) & 0xFFFFFFFFFFFFFFFF for j in range(4)], dtype=np.uint64)
+
+
+def pairing_is_one(eng, curve, g1_points, g2_points):
+    """prod_i e(g1_points[i], g2_points[i]) == 1 as one equation of pcgpu_multi_pairing; points are (xy, is_identity) pairs"""
+    g1 = np.stack([xy for xy, _ in g1_points])
+    g2 = np.stack([xy for xy, _ in g2_points])
+    g1_inf = np.array([inf for _, inf in g1_points], dtype=np.uint8)
+    g2_inf = np.array([inf for _, inf in g2_points], dtype=np.uint8)
+    _, one = eng.multi_pairing(curve, g1, g2, len(g1_points), g1_inf=g1_inf, g2_inf=g2_inf)
+    return bool(one[0])
+
+
+def check(eng, curve, vk, comm, point, value, proof_w, random_v=None):
+    """KZG10::check (kzg10/mod.rs:314-333): comm and proof_w are G1 xy rows or (xy, is_identity); point, value, random_v:
+    (4,) Montgomery Fr.  The G2 side beta_h - point * h is one two-term G2 MSM."""
+    comm, _ = _point(comm)
+    w_xy, w_inf = _point(proof_w)
+    inner = check_inner(eng, curve, vk["g"], vk["gamma_g"], comm, value, random_v)
+    h = np.asarray(vk["h"], dtype=np.uint64).reshape(-1)
+    rhs_g2 = eng.msm_bases(G2_OF[curve], np.stack([np.asarray(vk["beta_h"], dtype=np.uint64).reshape(-1), h]),
+                           np.stack([_one_mont(curve), _neg_limbs(point, FR_MODULUS[curve])]), flags=SCALARS_MONT)
+    neg_w = (np.zeros_like(w_xy), True) if w_inf else (neg_point(curve, w_xy), False)
+    return pairing_is_one(eng, curve, [inner, neg_w], [(h, False), rhs_g2])
+
+
+def batch_check(eng, curve, vk, commitments, points, values, proofs_w, randomizers, random_vs=None):
+    """KZG10::batch_check (kzg10/mod.rs:337-391) with the randomizers as an argument (batch_check_combine)"""
+    neg_w, total_c = batch_check_combine(eng, curve, vk["g"], vk["gamma_g"], commitments, points, values, proofs_w, randomizers,
+                                         random_vs)
+    return pairing_is_one(eng, curve, [neg_w, total_c], [(np.asarray(vk["beta_h"], dtype=np.uint64).reshape(-1), False),
+                                                          (np.asarray(vk["h"], dtype=np.uint64).reshape(-1), False)])

@@ -9,6 +9,10 @@ degree-bound branches included.
                                                                           witness :292-297, shifted_w / shifted_r / shifted_r_witness
                                                                           :300-307, KZG10::open :310, shifted opening :317-326
 
+Verifier side (the G1 combinations on device MSMs, the pairings on pcgpu_multi_pairing):
+  check        marlin_pc/mod.rs:340-364   accumulate_commitments_and_values, then KZG10::check
+  batch_check  marlin_pc/mod.rs:366-398   combine_and_normalize (marlin/mod.rs:151-219), then KZG10::batch_check
+
 The opening challenges are squeezed from a Poseidon sponge in the reference (:282, :299) and the blinding polynomials are
 sampled from its RNG (kzg10/mod.rs:182-195); here both are arguments (sponge and RNG are out of scope, SURVEY.md section 2)
 -- they are data to the kernels.  Polynomials are (n, 4) uint64 arrays of Montgomery Fr coefficients, low degree first.
@@ -200,3 +204,41 @@ def accumulate_commitments_and_values(eng, curve, commitments, values, challenge
             scalars += [c1, _neg_limbs(c1v, FR_MODULUS[curve])]
     combined_value = eng.fr_inner_product(curve, np.stack(ch_plain), values[: len(ch_plain)])
     return eng.msm_bases(curve, np.stack(bases), np.stack(scalars), flags=SCALARS_MONT), combined_value
+
+
+def check(eng, curve, vk, commitments, point, values, proof, challenges, shift_powers=None):
+    """MarlinKZG10::check (marlin_pc/mod.rs:340-364).  vk: the KZG10 verifier key dict (kzg10.check); commitments, values,
+    challenges, shift_powers as in accumulate_commitments_and_values; point: (4,) Montgomery Fr; proof: (w_xy or (w_xy,
+    is_identity), random_v or None)."""
+    from . import kzg10
+    comm, value = accumulate_commitments_and_values(eng, curve, commitments, values, challenges, shift_powers)
+    return kzg10.check(eng, curve, vk, comm, point, value, proof[0], proof[1])
+
+
+def batch_check(eng, curve, vk, commitments, query_set, evaluations, proofs, challenges, randomizers, shift_powers=None):
+    """MarlinKZG10::batch_check (marlin_pc/mod.rs:366-398).  commitments: {label: (comm_xy, shifted_xy or None, degree_bound or
+    None)}; query_set: iterable of (label, (point_label, point)); evaluations: {(label, point_label): value}; proofs: one
+    (w, random_v or None) per distinct point label, in point-label order; challenges: the sponge's challenges in the order
+    combine_and_normalize draws them; randomizers: one (4,) Montgomery Fr per distinct point (the first is 1 in the reference).
+    Queries are grouped by point label and each group's labels taken in sorted order (marlin/mod.rs:151-219)."""
+    from . import kzg10
+    groups = {}
+    for label, (point_label, point) in query_set:
+        groups.setdefault(point_label, (point, set()))[1].add(label)
+    ch = iter(challenges)
+    combined, points, values = [], [], []
+    for point_label in sorted(groups):
+        point, labels = groups[point_label]
+        labels = sorted(labels)
+        vals = np.stack([np.asarray(evaluations[(lb, point_label)], dtype=np.uint64).reshape(4) for lb in labels])
+        (c_xy, c_inf), v = accumulate_commitments_and_values(eng, curve, [commitments[lb] for lb in labels], vals, ch, shift_powers)
+        if c_inf:
+            raise ValueError("combined commitment is the identity")
+        combined.append(c_xy); points.append(np.asarray(point, dtype=np.uint64).reshape(4)); values.append(np.asarray(v).reshape(4))
+    ws = [kzg10._point(w)[0] for w, _ in proofs]
+    rvs = [rv for _, rv in proofs]
+    hiding = any(rv is not None for rv in rvs)
+    random_vs = np.stack([np.zeros(4, dtype=np.uint64) if rv is None else np.asarray(rv, dtype=np.uint64).reshape(4) for rv in rvs]) \
+        if hiding else None
+    return kzg10.batch_check(eng, curve, vk, np.stack(combined), np.stack(points), np.stack(values), np.stack(ws), randomizers,
+                             random_vs)

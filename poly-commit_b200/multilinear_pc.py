@@ -5,6 +5,8 @@
   trim    :91-111   drop the first num_vars - nv levels
   commit  :114-128  one G1 MSM over powers_of_g[0] with the evaluations as scalars (pcgpu_msm, SCALARS_MONT)
   open    :131-168  fold chain and nv G2 MSMs on the device (pcgpu_mlpc_open over a key with pair-folded powers_of_h)
+  check   :172-200  e(comm - g value, h) == prod_i e(g_mask_i - point_i g, proof_i), as one equation of nv + 1 pairs
+                    e(comm - g value, h) * prod_i e(point_i g - g_mask_i, proof_i) == 1 (G1 side: pcgpu_msm_bases)
 
 The reference samples t, g and h from its RNG; here they are inputs (the Rust RNG is not reproducible outside Rust).  Scalars
 are plain ints below r (t) or (.., 4) uint64 Montgomery Fr (evaluations, point); points are Montgomery limb rows.
@@ -13,6 +15,8 @@ import numpy as np
 
 from .binding import G2_OF, SCALARS_MONT
 from .params import FR_MODULUS
+
+_U64 = 0xFFFFFFFFFFFFFFFF
 
 
 def eq_extension(t, r):
@@ -106,3 +110,32 @@ class Committer:
     def release(self):
         self.g_srs.release()
         self.h_key.release()
+
+
+def check(eng, curve, vk, comm, point, value, proofs):
+    """MultilinearPC::check (:172-200).  vk from trim; comm: Commitment.g_product as xy or (xy, is_identity); point: (nv, 4)
+    Montgomery Fr; value: (4,) Montgomery Fr; proofs: (proofs_xy (nv, 4*limbs), identity flags (nv,) or None) as
+    Committer.open returns them."""
+    r = FR_MODULUS[curve]
+
+    def neg(x):
+        v = sum(int(w) << (64 * j) for j, w in enumerate(np.asarray(x, dtype=np.uint64).reshape(-1)))
+        v = (r - v) % r
+        return np.array([(v >> (64 * j)) & _U64 for j in range(4)], dtype=np.uint64)
+
+    one = np.array([((1 << 256) % r >> (64 * j)) & _U64 for j in range(4)], dtype=np.uint64)
+    nv = vk["nv"]
+    g = np.asarray(vk["g"], dtype=np.uint64).reshape(-1)
+    comm_xy = np.asarray(comm[0] if isinstance(comm, tuple) else comm, dtype=np.uint64).reshape(-1)
+    point = np.asarray(point, dtype=np.uint64).reshape(nv, 4)
+    g1 = [eng.msm_bases(curve, np.stack([comm_xy, g]), np.stack([one, neg(value)]), flags=SCALARS_MONT)]
+    for i in range(nv):
+        mask = np.asarray(vk["g_mask_random"][i], dtype=np.uint64).reshape(-1)
+        g1.append(eng.msm_bases(curve, np.stack([mask, g]), np.stack([neg(one), point[i]]), flags=SCALARS_MONT))
+    proofs_xy = np.asarray(proofs[0], dtype=np.uint64).reshape(nv, -1)
+    pinf = np.zeros(nv, dtype=np.uint8) if len(proofs) < 2 or proofs[1] is None else np.asarray(proofs[1], dtype=np.uint8)
+    g2 = np.concatenate([np.asarray(vk["h"], dtype=np.uint64).reshape(1, -1), proofs_xy])
+    g1_xy = np.stack([xy for xy, _ in g1])
+    g1_inf = np.array([inf for _, inf in g1], dtype=np.uint8)
+    _, ok = eng.multi_pairing(curve, g1_xy, g2, nv + 1, g1_inf=g1_inf, g2_inf=np.concatenate([[0], pinf]).astype(np.uint8))
+    return bool(ok[0])

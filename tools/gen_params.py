@@ -127,6 +127,57 @@ def glv_consts(c):
 
 
 BLS_X = 0xd201000000010000          # |z| of BLS12-381 (z is negative); ark-bls12-381 `Config::X`
+BN_U = 4965661367192848881          # u of BN254 (positive); the optimal-ate loop runs over 6u + 2
+
+
+def fq2_mul(a, b, p):
+    return ((a[0] * b[0] - a[1] * b[1]) % p, (a[0] * b[1] + a[1] * b[0]) % p)
+
+
+def fq2_pow(a, e, p):
+    acc = (1, 0)
+    for bit in bin(e)[2:]:
+        acc = fq2_mul(acc, acc, p)
+        if bit == "1":
+            acc = fq2_mul(acc, a, p)
+    return acc
+
+
+def pairing_consts(cname, c):
+    """Constants of the optimal-ate pairing over the tower Fq2 = Fq[u]/(u^2 + 1), Fq6 = Fq2[v]/(v^3 - xi),
+    Fq12 = Fq6[w]/(w^2 - v) (pairing.cuh): xi, the twist's 3 b', the Frobenius coefficients, the Miller loop scalar and the
+    joint base-p digits of the hard part of the final exponentiation."""
+    p, r = c["p"], c["r"]
+    xi0 = 1 if cname == "bls12_381" else 9
+    xi = (xi0, 1)
+    if cname == "bls12_381":      # M-type twist y^2 = x^3 + b xi
+        b2 = (4 * xi[0] % p, 4 * xi[1] % p)
+        loop, neg, frob = BLS_X, 1, 0
+    else:                         # D-type twist y^2 = x^3 + b / xi
+        n = pow(xi0 * xi0 + 1, -1, p)
+        b2 = (3 * xi0 * n % p, (-3 * n) % p)
+        loop, neg, frob = 6 * BN_U + 2, 0, 1
+    assert (p - 1) % 6 == 0
+    # a^(p^k) of c0 + c1 v + c2 v^2 scales c1 by xi^((p^k - 1) / 3) and c2 by xi^(2 (p^k - 1) / 3); of c0 + c1 w scales c1 by
+    # xi^((p^k - 1) / 6)
+    frob_tab = []
+    for k in (1, 2, 3):
+        e = p ** k - 1
+        frob_tab += [fq2_pow(xi, e // 3, p), fq2_pow(xi, 2 * e // 3, p), fq2_pow(xi, e // 6, p)]
+    # pi on the D-type twist: (x, y) -> (conj(x) xi^((p - 1) / 3), conj(y) xi^((p - 1) / 2))
+    tw_x, tw_y = fq2_pow(xi, (p - 1) // 3, p), fq2_pow(xi, (p - 1) // 2, p)
+    # hard part: e = (p^4 - p^2 + 1) / r exactly, as sum lambda_i p^i with 0 <= lambda_i < p; digit j packs bit j of lambda_i
+    # at bit i
+    hard = (p ** 4 - p ** 2 + 1)
+    assert hard % r == 0
+    hard //= r
+    lam = [(hard // p ** i) % p for i in range(4)]
+    assert sum(l * p ** i for i, l in enumerate(lam)) == hard
+    bits = max(l.bit_length() for l in lam)
+    digits = [sum(((lam[i] >> j) & 1) << i for i in range(4)) for j in range(bits)]
+    words = [sum(digits[j] << (4 * (j - 8 * w)) for j in range(8 * w, min(8 * w + 8, bits))) for w in range((bits + 7) // 8)]
+    return dict(xi0=xi0, twist_m=1 if cname == "bls12_381" else 0, b3=(3 * b2[0] % p, 3 * b2[1] % p), frob=frob_tab,
+                tw_x=tw_x, tw_y=tw_y, loop=loop, loop_neg=neg, loop_frob=frob, hard_bits=bits, hard_words=words)
 
 
 def check_curve(c):
@@ -199,6 +250,31 @@ def main():
             extra_q += arrq("beta", 0) + "  static constexpr unsigned long long SUBGROUP_X = 0ull;\n  static constexpr int COFACTOR_ONE = 1;\n"
         nr = fr["n32"]
         extra_r = arrq("root_of_unity", root * Rr % r, nr) + f"  static constexpr int TWO_ADICITY = {c['two_adicity']};\n"
+        if cname in ("bls12_381", "bn254"):
+            pc = pairing_consts(cname, c)
+
+            def arrq2(fn, vals):
+                """Fq2 constants, Montgomery: entry j holds c0 in words 0..N-1 and c1 in words N..2N-1"""
+                rows = ["{" + fmt(limbs(v[0] * Rq % p, n, 32) + limbs(v[1] * Rq % p, n, 32), 32) + "}" for v in vals]
+                return (f"  PCGPU_HD static constexpr uint32_t {fn}(int j, int i) {{\n"
+                        f"    constexpr uint32_t v[{len(vals)}][{2 * n}] = {{{', '.join(rows)}}};\n    return v[j][i];\n  }}\n")
+            lw = [(pc["loop"] >> (32 * i)) & 0xFFFFFFFF for i in range((pc["loop"].bit_length() + 31) // 32)]
+            extra_q += ("  // optimal-ate pairing (pairing.cuh): xi = XI0 + u; TWIST_M: M-type twist (else D-type)\n"
+                        f"  static constexpr int XI0 = {pc['xi0']};\n  static constexpr int TWIST_M = {pc['twist_m']};\n")
+            extra_q += "  // 3 b' of the twist\n" + arrq2("twist_b3", [pc["b3"]])
+            extra_q += ("  // Frobenius a^(p^k), k = 1, 2, 3: entry 3 (k - 1) + 0 / 1 scales Fq6's v / v^2 coefficient, + 2 scales Fq12's w"
+                        " coefficient\n") + arrq2("frob", pc["frob"])
+            extra_q += "  // pi on the twist: x scales by entry 0, y by entry 1 (after conjugation)\n" + arrq2("twist_frob", [pc["tw_x"], pc["tw_y"]])
+            extra_q += (f"  // Miller loop scalar (|x| for BLS12-381, 6u + 2 for BN254), its bit length, 32-bit words low first\n"
+                        f"  static constexpr int MILLER_BITS = {pc['loop'].bit_length()};\n"
+                        f"  static constexpr int MILLER_NEG = {pc['loop_neg']};\n  static constexpr int MILLER_FROB = {pc['loop_frob']};\n"
+                        f"  PCGPU_HD static constexpr uint32_t miller_loop(int i) {{\n"
+                        f"    constexpr uint32_t v[{len(lw)}] = {{{fmt(lw, 32)}}};\n    return v[i];\n  }}\n")
+            hw = pc["hard_words"]
+            extra_q += (f"  // hard part (p^4 - p^2 + 1) / r = sum_i lambda_i p^i: 4-bit digit j (8 per word) has bit i = bit j of lambda_i\n"
+                        f"  static constexpr int HARD_BITS = {pc['hard_bits']};\n"
+                        f"  PCGPU_HD static constexpr uint32_t hard_digits(int i) {{\n"
+                        f"    constexpr uint32_t v[{len(hw)}] = {{{fmt(hw, 32)}}};\n    return v[i];\n  }}\n")
         gl = glv_consts(c)
         extra_q += "  // GLV endomorphism phi(x, y) = (glv_zeta x, y) = [glv_lambda] (x, y)  (ipa.cuh key folding)\n" + arrq("glv_zeta", gl["zeta"] * Rq % p)
         extra_r += "  // GLV: lambda (Montgomery) and the lattice basis |a1|, |b1|, |a2|, |b2| (128-bit magnitudes) with their signs\n"
