@@ -77,7 +77,7 @@ int pcgpu_set_stream(pcgpu_ctx *ctx, void *cuda_stream);
  * 2 scatter, 3 tasks, 4 bucket accumulate (XYZZ), 5 bucket reduce, 6 final (host tail, wall clock), 7 fr division,
  * 8 fr axpy, 9 ntt, 10 comb batch, 11 affine pair rounds (all), 12 affine pair round 0 kernel alone, 13 peer push + wait,
  * 14 column hashes + Merkle tree, 15 Brakedown encoding, 16 MultilinearPC open fold chain, 17 pairing Miller loops + final
- * exponentiations.
+ * exponentiations (prepared or not), 18 G2 line preparation.
  * enable=1 starts recording; get returns accumulated milliseconds and launch count since enable. */
 int pcgpu_profile_enable(pcgpu_ctx *ctx, int enable);
 int pcgpu_profile_get(pcgpu_ctx *ctx, int stage, double *ms, uint64_t *count);
@@ -357,6 +357,26 @@ int pcgpu_mlpc_open(pcgpu_ctx *ctx, const pcgpu_mlpc *key, const void *evals, si
 #define PCGPU_PAIRING_MAX_K 64
 int pcgpu_multi_pairing(pcgpu_ctx *ctx, int curve, const void *g1_xy, const uint8_t *g1_inf, const void *g2_xy,
                         const uint8_t *g2_inf, size_t k, size_t count, uint32_t flags, void *out_gt, uint8_t *out_is_one);
+
+/* Prepared G2 points (ark's G2Prepared): the Miller loop's line coefficients of n fixed G2 points, computed once and kept on
+ * the device, so pairings against them skip the twist arithmetic -- a verifier key's h, beta_h and degree-bound powers.
+ *   pcgpu_g2_prepare: curve PCGPU_BLS12_381 or PCGPU_BN254 (any other id, G2 ids included: PCGPU_E_BADARG); g2_xy: n G2
+ *   affine points (x.c0 x.c1 y.c0 y.c1), g2_inf: their identity bytes or NULL (an identity, or the all-zero encoding, makes
+ *   its pairs contribute 1); with PCGPU_DEVICE_PTRS both are device pointers.  Points are NOT validated, as in
+ *   G2Prepared::from.  About 19 KB of lines per point (68 lines on BLS12-381, 100 on BN254).  *out is cleared whenever out is non-null.
+ *   Profile stage 18.
+ *   pcgpu_multi_pairing_prepared: pcgpu_multi_pairing with equation j = prod_{i<k} e(P[j*k+i], Q[q_index[j*k+i]]) over the
+ *   handle's points.  g1_xy / g1_inf as in pcgpu_multi_pairing (device pointers with PCGPU_DEVICE_PTRS); q_index: k * count
+ *   indices, a host array in every mode, checked before anything runs (an index >= n: PCGPU_E_BADARG).  A handle prepared on
+ *   another curve: PCGPU_E_BADARG.  Outputs, k == 0, count == 0 and PCGPU_PAIRING_MAX_K as in pcgpu_multi_pairing; profile
+ *   stage 17. */
+typedef struct pcgpu_g2_prepared pcgpu_g2_prepared;
+int pcgpu_g2_prepare(pcgpu_ctx *ctx, int curve, const void *g2_xy, const uint8_t *g2_inf, size_t n, uint32_t flags,
+                     pcgpu_g2_prepared **out);
+void pcgpu_g2_prepared_release(pcgpu_ctx *ctx, pcgpu_g2_prepared *q);
+int pcgpu_multi_pairing_prepared(pcgpu_ctx *ctx, int curve, const void *g1_xy, const uint8_t *g1_inf, const pcgpu_g2_prepared *q,
+                                 const uint32_t *q_index, size_t k, size_t count, uint32_t flags, void *out_gt,
+                                 uint8_t *out_is_one);
 
 /* ---- KZG10 fused prover calls ------------------------------------------------------------------ */
 /* KZG10::commit -- kzg10/mod.rs:157-210.  coeffs: n Montgomery Fr (low degree first; trailing zeros allowed and

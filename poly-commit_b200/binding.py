@@ -102,6 +102,9 @@ def _load(path):
         "pcgpu_msm_last_geometry": [_vp, ctypes.POINTER(ctypes.c_uint64), _sz],
         "pcgpu_diag_field_op": [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp, _sz],
         "pcgpu_multi_pairing": [_vp, ctypes.c_int, _vp, _vp, _vp, _vp, _sz, _sz, ctypes.c_uint32, _vp, _vp],
+        "pcgpu_g2_prepare": [_vp, ctypes.c_int, _vp, _vp, _sz, ctypes.c_uint32, ctypes.POINTER(_vp)],
+        "pcgpu_g2_prepared_release": [_vp, _vp],
+        "pcgpu_multi_pairing_prepared": [_vp, ctypes.c_int, _vp, _vp, _vp, _vp, _sz, _sz, ctypes.c_uint32, _vp, _vp],
         "pcgpu_ipa_begin": [_vp, ctypes.c_int, _vp, _sz, _vp, _sz, _vp, ctypes.c_uint32, ctypes.POINTER(_vp)],
         "pcgpu_ipa_round_lr": [_vp, _vp, _vp, _vp, _vp, _vp, _vp],
         "pcgpu_ipa_round_fold": [_vp, _vp, _vp, _vp],
@@ -150,8 +153,8 @@ def _load(path):
         if fn is None:      # a library older than this binding: only the calls that need the symbol fail (AttributeError)
             continue
         fn.argtypes = args
-        fn.restype = None if name in ("pcgpu_destroy", "pcgpu_srs_release", "pcgpu_brakedown_release", "pcgpu_mlpc_release") \
-            else ctypes.c_int
+        fn.restype = None if name in ("pcgpu_destroy", "pcgpu_srs_release", "pcgpu_brakedown_release", "pcgpu_mlpc_release",
+                                      "pcgpu_g2_prepared_release") else ctypes.c_int
     return lib
 
 
@@ -226,6 +229,19 @@ class MlpcKey(_Handle):
 
     def _free(self, h, ctx):
         self.engine.lib.pcgpu_mlpc_release(ctx, h)
+
+
+class G2Prepared(_Handle):
+    """Device-resident Miller lines of n fixed G2 points (ark's G2Prepared), for multi_pairing_prepared."""
+
+    def __init__(self, engine, handle, curve, n):
+        self.engine, self.handle, self.curve, self.n = engine, handle, curve, n
+
+    def __len__(self):
+        return self.n
+
+    def _free(self, h, ctx):
+        self.engine.lib.pcgpu_g2_prepared_release(ctx, h)
 
 
 class DeviceBuffer(_Handle):
@@ -367,6 +383,33 @@ class Engine:
         one = np.zeros(count, dtype=np.uint8)
         self._ck(self.lib.pcgpu_multi_pairing(self.ctx, curve, _ptr(g1), _ptr(g1_inf), _ptr(g2), _ptr(g2_inf), k, count, flags,
                                               _ptr(gt), _ptr(one)))
+        return gt, one
+
+    def g2_prepare(self, curve, g2_xy, g2_inf=None, n=None, flags=0):
+        """G2Prepared::from for each of the (n, 4*limbs) G2 affine points (pcgpu_g2_prepare); g2_inf: None or identity bytes.
+        With DEVICE_PTRS both are device pointers and n must be given."""
+        g2_xy = _u64(g2_xy)
+        if n is None:
+            n = g2_xy.size // (4 * fq_limbs(curve))
+        if g2_inf is not None and not isinstance(g2_inf, (int, np.integer)):
+            g2_inf = np.ascontiguousarray(g2_inf, dtype=np.uint8)
+        h = _vp()
+        self._ck(self.lib.pcgpu_g2_prepare(self.ctx, curve, _ptr(g2_xy), _ptr(g2_inf), n, flags, ctypes.byref(h)))
+        return G2Prepared(self, h, curve, n)
+
+    def multi_pairing_prepared(self, curve, g1, prepared, q_index, k, g1_inf=None, flags=0, count=None):
+        """multi_pairing with pair i taken as (g1[i], prepared point q_index[i]) (pcgpu_multi_pairing_prepared); q_index is a
+        host array in every mode.  Shapes, count and the result as in multi_pairing."""
+        g1 = _u64(g1)
+        if count is None:
+            count = (g1.size // (2 * fq_limbs(curve))) // k if k else 1
+        if g1_inf is not None and not isinstance(g1_inf, (int, np.integer)):
+            g1_inf = np.ascontiguousarray(g1_inf, dtype=np.uint8)
+        q_index = np.ascontiguousarray(q_index, dtype=np.uint32) if q_index is not None else None
+        gt = np.zeros((count, 12 * fq_limbs(curve)), dtype=np.uint64)
+        one = np.zeros(count, dtype=np.uint8)
+        self._ck(self.lib.pcgpu_multi_pairing_prepared(self.ctx, curve, _ptr(g1), _ptr(g1_inf), prepared.handle, _ptr(q_index), k,
+                                                       count, flags, _ptr(gt), _ptr(one)))
         return gt, one
 
     # ---- SRS ----

@@ -34,6 +34,7 @@ static void free_device(pcgpu_srs *srs) { rt::dev_free(srs->d_tables); rt::dev_f
 static void free_device(pcgpu_mlpc *key) { free_device(&key->key); }
 static void free_device(pcgpu_brakedown *code) { rt::dev_free(code->d_mem); }
 static void free_device(pcgpu_ipa *) {}
+static void free_device(pcgpu_g2_prepared *q) { rt::dev_free(q->d_lines); }
 
 // Every creating entry point: *out is cleared whenever out is non-null, then make(handle) fills a fresh handle under the
 // context's lock.  *out receives the handle only when make succeeds; on failure its device memory is freed and it is deleted.
@@ -252,6 +253,29 @@ extern "C" int pcgpu_multi_pairing(pcgpu_ctx *ctx, int curve, const void *g1_xy,
                         (flags & ~(uint32_t)PCGPU_DEVICE_PTRS);
   return on_ctx(ctx, bad_args, [&]() -> int {
     DISPATCH_PAIRING(curve, return multi_pairing_impl<C>(ctx, g1_xy, g1_inf, g2_xy, g2_inf, k, count, flags, out_gt, out_is_one));
+  });
+}
+
+extern "C" int pcgpu_g2_prepare(pcgpu_ctx *ctx, int curve, const void *g2_xy, const uint8_t *g2_inf, size_t n, uint32_t flags,
+                                pcgpu_g2_prepared **out) {
+  const bool bad_args = (n && !g2_xy) || n > UINT32_MAX || (flags & ~(uint32_t)PCGPU_DEVICE_PTRS);
+  return create(ctx, bad_args, out, [&](pcgpu_g2_prepared *q) -> int {
+    q->curve = curve; q->n = n;
+    DISPATCH_PAIRING(curve, return g2_prepare_impl<C>(ctx, g2_xy, g2_inf, n, flags, q));
+  });
+}
+
+extern "C" void pcgpu_g2_prepared_release(pcgpu_ctx *ctx, pcgpu_g2_prepared *q) { release_after_stream(ctx, q); }
+
+extern "C" int pcgpu_multi_pairing_prepared(pcgpu_ctx *ctx, int curve, const void *g1_xy, const uint8_t *g1_inf,
+                                            const pcgpu_g2_prepared *q, const uint32_t *q_index, size_t k, size_t count,
+                                            uint32_t flags, void *out_gt, uint8_t *out_is_one) {
+  bool bad_args = !q || q->curve != curve || k > PCGPU_PAIRING_MAX_K || (!out_gt && !out_is_one) ||
+                  (k && count && (!g1_xy || !q_index)) || (flags & ~(uint32_t)PCGPU_DEVICE_PTRS);
+  if (!bad_args && k && count)   // every index names a prepared point before anything runs
+    for (size_t i = 0; i < k * count && !bad_args; i++) bad_args = q_index[i] >= q->n;
+  return on_ctx(ctx, bad_args, [&]() -> int {
+    DISPATCH_PAIRING(curve, return multi_pairing_prepared_impl<C>(ctx, g1_xy, g1_inf, q, q_index, k, count, flags, out_gt, out_is_one));
   });
 }
 

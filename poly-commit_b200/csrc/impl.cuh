@@ -35,7 +35,7 @@ using namespace pcgpu;
 // ---------------------------------------------------------------------------------------------
 // profiling (CUDA events on the launching stream)
 // ---------------------------------------------------------------------------------------------
-enum { PROF_STAGES = 18 };
+enum { PROF_STAGES = 19 };
 struct Prof {
   bool on = false;
   double ms[PROF_STAGES] = {0};
@@ -1873,6 +1873,65 @@ int multi_pairing_impl(pcgpu_ctx *ctx, const void *g1_xy, const uint8_t *g1_inf,
   return rt::stream_sync(st);
 }
 
+// pcgpu_g2_prepare: every point's Miller lines in one device allocation, the identity flags after them
+struct pcgpu_g2_prepared {
+  int curve = 0;        // the pairing curve (PCGPU_BLS12_381 / PCGPU_BN254)
+  size_t n = 0;
+  uint32_t *d_lines = nullptr;
+  uint8_t *d_inf = nullptr;   // inside d_lines' allocation
+};
+
+template <class C>
+int g2_prepare_impl(pcgpu_ctx *ctx, const void *g2_xy, const uint8_t *g2_inf, size_t n, uint32_t flags, pcgpu_g2_prepared *h) {
+  using P = typename C::Fq;
+  if (n == 0) return PCGPU_OK;
+  rt::stream_t st = ctx->stream;
+  const size_t line_bytes = n * prepared_point_words<P>() * 4;
+  int rc;
+  if ((rc = rt::dev_malloc((void **)&h->d_lines, line_bytes + n))) return rc;
+  h->d_inf = (uint8_t *)h->d_lines + line_bytes;
+  const uint32_t *d_g2 = nullptr;
+  const uint8_t *d_g2_inf = nullptr;
+  Staging io(ctx, flags);
+  io.in(d_g2, g2_xy, n * 4 * P::N * 4);
+  if (g2_inf) io.in(d_g2_inf, g2_inf, n);
+  if ((rc = io.upload())) return rc;
+  ctx->prof.begin(18, st);
+  if ((rc = rt::launch<64>(G2PrepareBody<P>{d_g2, d_g2_inf, h->d_lines, h->d_inf}, n, st))) return rc;
+  ctx->prof.end(18, st);
+  return rt::stream_sync(st);
+}
+
+// pcgpu_multi_pairing_prepared: multi_pairing_impl with the Miller values read from prepared lines (q_index range-checked by
+// the caller)
+template <class C>
+int multi_pairing_prepared_impl(pcgpu_ctx *ctx, const void *g1_xy, const uint8_t *g1_inf, const pcgpu_g2_prepared *q,
+                                const uint32_t *q_index, size_t k, size_t count, uint32_t flags, void *out_gt, uint8_t *out_is_one) {
+  using P = typename C::Fq;
+  if (count == 0) return PCGPU_OK;
+  rt::stream_t st = ctx->stream;
+  const size_t pairs = k * count;
+  int rc;
+  const uint32_t *d_g1 = nullptr, *d_index = nullptr;
+  const uint8_t *d_g1_inf = nullptr;
+  uint32_t *d_miller, *d_gt;
+  uint8_t *d_one;
+  Staging io(ctx, flags);
+  io.in(d_g1, g1_xy, pairs * 2 * P::N * 4);
+  if (g1_inf) io.in(d_g1_inf, g1_inf, pairs);
+  io.host_in(d_index, q_index, pairs * 4);
+  io.scratch(d_miller, pairs * Fq12<P>::WORDS * 4);
+  io.host_out(d_gt, out_gt, count * Fq12<P>::WORDS * 4);
+  io.host_out(d_one, out_is_one, count);
+  if ((rc = io.upload())) return rc;
+  ctx->prof.begin(17, st);
+  if ((rc = rt::launch<64>(MillerPreparedBody<P>{d_g1, d_g1_inf, q->d_lines, q->d_inf, d_index, d_miller}, pairs, st))) return rc;
+  if ((rc = rt::launch<64>(FinalExpBody<P>{d_miller, k, d_gt, d_one}, count, st))) return rc;
+  ctx->prof.end(17, st);
+  if ((rc = io.download())) return rc;
+  return rt::stream_sync(st);
+}
+
 template <class C>
 int diag_field_op_impl(pcgpu_ctx *ctx, int which, int op, const void *a, const void *b, void *out, size_t n) {
   if (n == 0) return PCGPU_OK;
@@ -2026,7 +2085,10 @@ inline int measure_imad_peak_impl(pcgpu_ctx *ctx, double *ops_per_s) {
 #define PCGPU_INST_PAIRING(C, EXT)                                                                                         \
   EXT template int multi_pairing_impl<C>(pcgpu_ctx *, const void *, const uint8_t *, const void *, const uint8_t *, size_t, size_t, \
                                          uint32_t, void *, uint8_t *);                                                     \
-  EXT template int diag_fq12_op_impl<C>(pcgpu_ctx *, int, const void *, const void *, void *, size_t);
+  EXT template int diag_fq12_op_impl<C>(pcgpu_ctx *, int, const void *, const void *, void *, size_t);                      \
+  EXT template int g2_prepare_impl<C>(pcgpu_ctx *, const void *, const uint8_t *, size_t, uint32_t, pcgpu_g2_prepared *);     \
+  EXT template int multi_pairing_prepared_impl<C>(pcgpu_ctx *, const void *, const uint8_t *, const pcgpu_g2_prepared *,   \
+                                                  const uint32_t *, size_t, size_t, uint32_t, void *, uint8_t *);
 #define PCGPU_INSTANTIATE_G2(C, EXT) \
   PCGPU_INST_ACC(C, EXT) PCGPU_INST_REDUCE(C, EXT) PCGPU_INST_PIPE(C, EXT) PCGPU_INST_SMALL(C, EXT) PCGPU_INST_G2(C, EXT)
 #define PCGPU_INSTANTIATE(C, EXT) \

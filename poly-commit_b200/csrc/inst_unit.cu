@@ -4,7 +4,8 @@
 //   5 IPA + wire   6 pair-round kernels   8 XYZZ accumulate   9 bucket reduction
 //   G2 of the pairing curves (BLS12-381, BN254) only: 10 pipeline host logic, small MSM, G2 / MultilinearPC entry points
 //   11 G2 XYZZ accumulate   12 G2 bucket reduction
-//   the pairing curves only: 13 the pairing (Miller loops, final exponentiations, Fq12 diagnostics)
+//   the pairing curves only: 13 the pairing (Miller loops plain and over prepared G2 lines, G2 line preparation, final
+//   exponentiations, Fq12 diagnostics)
 #include "impl.cuh"
 
 #ifndef PCGPU_UNIT_CURVE

@@ -15,6 +15,8 @@
 // for the chord through T and Q.  Vertical lines are dropped (the final exponentiation maps them to 1).
 //   BLS12-381: the loop runs over |x| = 0xd201000000010000, then f is conjugated (x < 0).
 //   BN254: the loop runs over 6u + 2, then the lines through pi(Q) and -pi^2(Q).
+// A fixed Q can be prepared once (ark's G2Prepared): G2PrepareBody walks the same loop with the same step functions and stores
+// every line; MillerPreparedBody then only squares f and folds the stored lines in at P.
 // Final exponentiation, one thread per equation: f^((p^6 - 1)(p^2 + 1)) by conjugation, inversion and Frobenius, then the hard
 // part (p^4 - p^2 + 1) / r exactly -- not a multiple of it, so GT values are those of the definition -- as
 // prod_i (f^(p^i))^lambda_i over the base-p digits lambda_i of the exponent, one joint square-and-multiply over a table of the
@@ -241,8 +243,7 @@ PCGPU_DEV_OUTLINE Fq12<P> fq12_mul_line(const Fq12<P> f, const Fq2<P> a, const F
 template <class P> struct G2Proj { Fq2<P> x, y, z; };
 template <class P> struct G2Aff { Fq2<P> x, y; };
 
-// f * line(T, T) at P, T <- 2T.  (X3 : Y3 : Z3) = (2 X Y (B - F), (B + F)^2 - 12 E^2, 4 B H) with B = Y^2, C = Z^2, E = 3 b' C,
-// F = 3 E, H = 2 Y Z: four times the usual doubling, which needs no halving
+// the line at P: its three coefficients scaled by yP / xP and folded into f with the sparse product of the twist
 template <class P>
 PCGPU_DEV Fq12<P> mul_line_at(const Fq12<P> &f, const Fq2<P> &ell0, const Fq2<P> &ell1, const Fq2<P> &ell2, const Fp<P> &xp,
                               const Fp<P> &yp) {
@@ -250,8 +251,13 @@ PCGPU_DEV Fq12<P> mul_line_at(const Fq12<P> &f, const Fq2<P> &ell0, const Fq2<P>
   else return fq12_mul_line<P>(f, fq2_mul_fp<P>(ell0, yp), fq2_mul_fp<P>(ell1, xp), ell2);
 }
 
+// one Miller line (ell0, ell1, ell2), independent of P
+template <class P> struct MillerLine { Fq2<P> ell0, ell1, ell2; };
+
+// T <- 2T and the tangent at T.  (X3 : Y3 : Z3) = (2 X Y (B - F), (B + F)^2 - 12 E^2, 4 B H) with B = Y^2, C = Z^2, E = 3 b' C,
+// F = 3 E, H = 2 Y Z: four times the usual doubling, which needs no halving
 template <class P>
-PCGPU_DEV_OUTLINE Fq12<P> miller_dbl(G2Proj<P> &T, const Fq12<P> f, const Fp<P> xp, const Fp<P> yp) {
+PCGPU_DEV MillerLine<P> dbl_step(G2Proj<P> &T) {
   const Fq2<P> B = fp_sqr<P>(T.y), C = fp_sqr<P>(T.z);
   const Fq2<P> E = fp_mul<P>(C, twist_b3_const<P>(0));
   const Fq2<P> F = fp_mul3<P>(E);
@@ -262,12 +268,12 @@ PCGPU_DEV_OUTLINE Fq12<P> miller_dbl(G2Proj<P> &T, const Fq12<P> f, const Fp<P> 
   T.x = fp_dbl<P>(fp_mul<P>(fp_mul<P>(T.x, T.y), fp_sub<P>(B, F)));
   T.y = fp_sub<P>(fp_sqr<P>(fp_add<P>(B, F)), fp_dbl<P>(fp_dbl<P>(fp_mul3<P>(e2))));
   T.z = fp_dbl<P>(fp_dbl<P>(fp_mul<P>(B, H)));
-  return mul_line_at<P>(f, fp_neg<P>(H), ell1, ell2, xp, yp);
+  return MillerLine<P>{fp_neg<P>(H), ell1, ell2};
 }
 
-// f * line(T, Q) at P, T <- T + Q (Q affine)
+// T <- T + Q (Q affine) and the chord through T and Q
 template <class P>
-PCGPU_DEV_OUTLINE Fq12<P> miller_add(G2Proj<P> &T, const G2Aff<P> Q, const Fq12<P> f, const Fp<P> xp, const Fp<P> yp) {
+PCGPU_DEV MillerLine<P> add_step(G2Proj<P> &T, const G2Aff<P> &Q) {
   const Fq2<P> theta = fp_sub<P>(T.y, fp_mul<P>(Q.y, T.z));
   const Fq2<P> lambda = fp_sub<P>(T.x, fp_mul<P>(Q.x, T.z));
   const Fq2<P> C = fp_sqr<P>(theta), D = fp_sqr<P>(lambda);
@@ -277,7 +283,21 @@ PCGPU_DEV_OUTLINE Fq12<P> miller_add(G2Proj<P> &T, const G2Aff<P> Q, const Fq12<
   T.x = fp_mul<P>(lambda, H);
   T.y = fp_sub<P>(fp_mul<P>(theta, fp_sub<P>(G, H)), fp_mul<P>(E, T.y));
   T.z = fp_mul<P>(T.z, E);
-  return mul_line_at<P>(f, lambda, fp_neg<P>(theta), ell2, xp, yp);
+  return MillerLine<P>{lambda, fp_neg<P>(theta), ell2};
+}
+
+// f * line(T, T) at P, T <- 2T
+template <class P>
+PCGPU_DEV_OUTLINE Fq12<P> miller_dbl(G2Proj<P> &T, const Fq12<P> f, const Fp<P> xp, const Fp<P> yp) {
+  const MillerLine<P> l = dbl_step<P>(T);
+  return mul_line_at<P>(f, l.ell0, l.ell1, l.ell2, xp, yp);
+}
+
+// f * line(T, Q) at P, T <- T + Q (Q affine)
+template <class P>
+PCGPU_DEV_OUTLINE Fq12<P> miller_add(G2Proj<P> &T, const G2Aff<P> Q, const Fq12<P> f, const Fp<P> xp, const Fp<P> yp) {
+  const MillerLine<P> l = add_step<P>(T, Q);
+  return mul_line_at<P>(f, l.ell0, l.ell1, l.ell2, xp, yp);
 }
 
 // pi on the D-type twist: (conj(x) xi^((p - 1) / 3), conj(y) xi^((p - 1) / 2))
@@ -305,6 +325,32 @@ PCGPU_DEV Fq12<P> miller_loop(const Fp<P> &xp, const Fp<P> &yp, const G2Aff<P> &
     f = miller_add<P>(T, q2, f, xp, yp);
   }
   return f;
+}
+
+// The lines miller_loop folds in for one Q, in its order: one tangent per step, one chord per set bit of the loop scalar
+// below the top bit, and the pi(Q) and -pi^2(Q) chords on BN254 -- ark's G2Prepared::ell_coeffs
+template <class P>
+PCGPU_HD constexpr int miller_line_count() {
+  int n = P::MILLER_FROB ? 2 : 0;
+  for (int i = P::MILLER_BITS - 2; i >= 0; i--) n += 1 + (int)((P::miller_loop(i / 32) >> (i % 32)) & 1);
+  return n;
+}
+// words of one prepared point: its lines, each ell0 ell1 ell2 as Fq2 Montgomery words
+template <class P> PCGPU_HD constexpr size_t prepared_point_words() { return (size_t)miller_line_count<P>() * 6 * P::N; }
+
+template <class P> PCGPU_DEV void line_store(uint32_t *dst, const MillerLine<P> &l) {
+#pragma unroll
+  for (int j = 0; j < 2 * P::N; j++) {
+    dst[j] = coord_word(l.ell0, j); dst[2 * P::N + j] = coord_word(l.ell1, j); dst[4 * P::N + j] = coord_word(l.ell2, j);
+  }
+}
+template <class P> PCGPU_DEV MillerLine<P> line_load(const uint32_t *src) {
+  MillerLine<P> l;
+#pragma unroll
+  for (int j = 0; j < 2 * P::N; j++) {
+    coord_word(l.ell0, j) = src[j]; coord_word(l.ell1, j) = src[2 * P::N + j]; coord_word(l.ell2, j) = src[4 * P::N + j];
+  }
+  return l;
 }
 
 // ---- final exponentiation: f^((p^12 - 1) / r) ----------------------------------------------------------------------------
@@ -342,6 +388,67 @@ struct MillerBody {
     for (int j = 0; j < 2 * N; j++) { coord_word(q.x, j) = g2[i * 4 * N + j]; coord_word(q.y, j) = g2[i * 4 * N + 2 * N + j]; }
     const bool inf = (g1_inf && g1_inf[i]) || (g2_inf && g2_inf[i]) || (xp.is_zero() && yp.is_zero()) || (q.x.is_zero() && q.y.is_zero());
     fq12_store<P>(out + i * Fq12<P>::WORDS, inf ? Fq12<P>::one() : miller_loop<P>(xp, yp, q));
+  }
+};
+
+// G2Prepared::from for point i: the lines of miller_loop over Q, in loop order, into lines[i * prepared_point_words]; inf[i]
+// is set for an identity flag or the all-zero encoding (its lines are not written: pairs with it contribute 1)
+template <class P>
+struct G2PrepareBody {
+  const uint32_t *g2; const uint8_t *g2_inf; uint32_t *lines; uint8_t *inf;
+  PCGPU_KERNEL_DEV void operator()(size_t i) const {
+    constexpr int N = P::N;
+    G2Aff<P> q;
+    for (int j = 0; j < 2 * N; j++) { coord_word(q.x, j) = g2[i * 4 * N + j]; coord_word(q.y, j) = g2[i * 4 * N + 2 * N + j]; }
+    inf[i] = (g2_inf && g2_inf[i]) || (q.x.is_zero() && q.y.is_zero());
+    if (inf[i]) return;
+    uint32_t *dst = lines + i * prepared_point_words<P>();
+    G2Proj<P> T{q.x, q.y, Fq2<P>::one()};
+    for (int b = P::MILLER_BITS - 2; b >= 0; b--) {
+      line_store<P>(dst, dbl_step<P>(T)); dst += 6 * N;
+      if ((P::miller_loop(b / 32) >> (b % 32)) & 1) { line_store<P>(dst, add_step<P>(T, q)); dst += 6 * N; }
+    }
+    if constexpr (P::MILLER_FROB) {
+      const G2Aff<P> q1 = twist_frob<P>(q);
+      G2Aff<P> q2 = twist_frob<P>(q1);
+      q2.y = fp_neg<P>(q2.y);
+      line_store<P>(dst, add_step<P>(T, q1)); dst += 6 * N;
+      line_store<P>(dst, add_step<P>(T, q2));
+    }
+  }
+};
+
+// MillerBody with Q prepared: pair i is g1 point i against prepared point q_index[i]; each step squares f and folds in the
+// stored lines, so T never lives in registers.  Writes MillerBody's output layout.
+template <class P>
+struct MillerPreparedBody {
+  const uint32_t *g1; const uint8_t *g1_inf; const uint32_t *lines; const uint8_t *q_inf; const uint32_t *q_index; uint32_t *out;
+  PCGPU_KERNEL_DEV void operator()(size_t i) const {
+    constexpr int N = P::N;
+    Fp<P> xp, yp;
+    for (int j = 0; j < N; j++) { xp.l[j] = g1[i * 2 * N + j]; yp.l[j] = g1[i * 2 * N + N + j]; }
+    const uint32_t q = q_index[i];
+    if ((g1_inf && g1_inf[i]) || q_inf[q] || (xp.is_zero() && yp.is_zero())) { fq12_store<P>(out + i * Fq12<P>::WORDS, Fq12<P>::one()); return; }
+    const uint32_t *src = lines + q * prepared_point_words<P>();
+    Fq12<P> f = Fq12<P>::one();
+    MillerLine<P> l;
+    for (int b = P::MILLER_BITS - 2; b >= 0; b--) {
+      f = fq12_sqr<P>(f);
+      l = line_load<P>(src); src += 6 * N;
+      f = mul_line_at<P>(f, l.ell0, l.ell1, l.ell2, xp, yp);
+      if ((P::miller_loop(b / 32) >> (b % 32)) & 1) {
+        l = line_load<P>(src); src += 6 * N;
+        f = mul_line_at<P>(f, l.ell0, l.ell1, l.ell2, xp, yp);
+      }
+    }
+    if constexpr (P::MILLER_NEG) f = fq12_conj<P>(f);
+    if constexpr (P::MILLER_FROB) {
+      for (int t = 0; t < 2; t++) {
+        l = line_load<P>(src); src += 6 * N;
+        f = mul_line_at<P>(f, l.ell0, l.ell1, l.ell2, xp, yp);
+      }
+    }
+    fq12_store<P>(out + i * Fq12<P>::WORDS, f);
   }
 };
 

@@ -252,6 +252,62 @@ def verifier_key_deserialize(eng, curve, data, compressed=True, validate=True):
     return dict(g=(xy[0], bool(inf[0])), gamma_g=(xy[1], bool(inf[1])), h=h, beta_h=beta_h, consumed=off)
 
 
+def sonic_verifier_key_serialize(eng, curve, g, gamma_g, h, beta_h, degree_bounds_and_neg_powers_of_h, supported_degree, max_degree,
+                                 compressed=True):
+    """SonicKZG10 VerifierKey::serialize_with_mode (sonic_pc/data_structures.rs:190-216): g, gamma_g, h, beta_h, then
+    Option<Vec<(usize, G2Affine)>> (a 1-byte tag, a u64 length, each bound as u64 and its point), supported_degree, max_degree"""
+    out = verifier_key_serialize(eng, curve, g, gamma_g, h, beta_h, compressed)
+    if degree_bounds_and_neg_powers_of_h is None:
+        out += b"\x00"
+    else:
+        out += b"\x01" + struct.pack("<Q", len(degree_bounds_and_neg_powers_of_h))
+        for bound, P in degree_bounds_and_neg_powers_of_h:
+            out += struct.pack("<Q", bound) + g2_host.g2_serialize(curve, P, compressed)
+    return out + struct.pack("<QQ", supported_degree, max_degree)
+
+
+def sonic_verifier_key_deserialize(eng, curve, data, compressed=True, validate=True):
+    """SonicKZG10 VerifierKey::deserialize_with_mode (sonic_pc/data_structures.rs:218-262) -> dict(g, gamma_g, h, beta_h,
+    degree_bounds_and_neg_powers_of_h=None or [(bound, point)], supported_degree, max_degree); Valid::check's
+    supported_degree > max_degree is InvalidData (:153-155)"""
+    data = bytes(data)
+    d = _Deferred()
+    sz = eng.g1_wire_size(curve, compressed)
+    if len(data) < 2 * sz:
+        raise ValueError("truncated input")
+    xy, inf = _g1_block(eng, curve, np.frombuffer(data, dtype=np.uint8, count=2 * sz), 2, compressed, validate, "g/gamma_g", d)
+    h, off = _g2_read(curve, data, 2 * sz, compressed, validate, "h", 0, d)
+    beta_h, off = _g2_read(curve, data, off, compressed, validate, "beta_h", 0, d)
+    if len(data) < off + 1:
+        raise ValueError("truncated input (option tag)")
+    tag, off = data[off], off + 1
+    if tag > 1:
+        raise ValueError("invalid option tag")
+    bounds = None
+    if tag:
+        if len(data) < off + 8:
+            raise ValueError("truncated input (vector length)")
+        (m,) = struct.unpack_from("<Q", data, off)
+        off += 8
+        bounds = []
+        for i in range(m):
+            if len(data) < off + 8:
+                raise ValueError("truncated input (degree bound)")
+            (b,) = struct.unpack_from("<Q", data, off)
+            P, off = _g2_read(curve, data, off + 8, compressed, validate, "degree_bounds_and_neg_powers_of_h", i, d)
+            bounds.append((b, P))
+    if len(data) < off + 16:
+        raise ValueError("truncated input (degrees)")
+    supported_degree, max_degree = struct.unpack_from("<QQ", data, off)
+    if d.first is not None:
+        raise KeyError_(*d.first)
+    if validate and supported_degree > max_degree:
+        raise ValueError("InvalidData: supported_degree > max_degree")
+    return dict(g=(xy[0], bool(inf[0])), gamma_g=(xy[1], bool(inf[1])), h=h, beta_h=beta_h,
+                degree_bounds_and_neg_powers_of_h=bounds, supported_degree=supported_degree, max_degree=max_degree,
+                consumed=off + 16)
+
+
 # ---- BrakedownPCParams (linear_codes/data_structures.rs:12-61), derived CanonicalSerialize -------------------------------
 # Field order of the struct; usize = u64 LE, Vec = u64 length + elements, tuples element by element, SprsMat = n, m, d,
 # ind_ptr, col_ind, val (linear_codes/utils.rs:20-37), Fr = 32 canonical LE bytes, bool = one byte.  The three hash
