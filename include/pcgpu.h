@@ -77,13 +77,14 @@ int pcgpu_set_stream(pcgpu_ctx *ctx, void *cuda_stream);
  * 2 scatter, 3 tasks, 4 bucket accumulate (XYZZ), 5 bucket reduce, 6 final (host tail, wall clock), 7 fr division,
  * 8 fr axpy, 9 ntt, 10 comb batch, 11 affine pair rounds (all), 12 affine pair round 0 kernel alone, 13 peer push + wait,
  * 14 column hashes + Merkle tree, 15 Brakedown encoding, 16 MultilinearPC open fold chain, 17 pairing Miller loops + final
- * exponentiations (prepared or not), 18 G2 line preparation.
+ * exponentiations (prepared or not), 18 G2 line preparation, 19 Hyrax transpose, tensors, row product and inner products.
  * enable=1 starts recording; get returns accumulated milliseconds and launch count since enable. */
 int pcgpu_profile_enable(pcgpu_ctx *ctx, int enable);
 int pcgpu_profile_get(pcgpu_ctx *ctx, int stage, double *ms, uint64_t *count);
 
 /* ---- SRS / committer key ---------------------------------------------------------------------- */
-/* The four creators -- pcgpu_srs_register, pcgpu_mlpc_register, pcgpu_brakedown_register, pcgpu_ipa_begin -- set *out to
+/* The creators -- pcgpu_srs_register, pcgpu_mlpc_register, pcgpu_brakedown_register, pcgpu_ipa_begin, pcgpu_g2_prepare,
+ * pcgpu_hyrax_commit -- set *out to
  * NULL whenever out is non-NULL, whatever they return, and store the new handle in it only on PCGPU_OK. */
 /* Upload n affine bases once (kzg10 Powers::powers_of_g, data_structures.rs:124-129; ipa CommitterKey::comm_key;
  * hyrax com_key).  inf may be NULL (no identity points).  `curve` may be a G2 group id: the key then holds raw G2 bases
@@ -175,7 +176,8 @@ int pcgpu_fr_div_linear(pcgpu_ctx *ctx, int curve, const void *p, size_t n, cons
                         uint32_t flags);
 /* <a, b> -- utils.rs:150-155.  out: host, 1 element */
 int pcgpu_fr_inner_product(pcgpu_ctx *ctx, int curve, const void *a, const void *b, size_t n, void *out, uint32_t flags);
-/* out = v * M, M rows x cols row-major -- Matrix::row_mul, utils.rs:127-146 */
+/* out = v * M, M rows x cols row-major -- Matrix::row_mul, utils.rs:127-146.  When the columns alone cannot fill the device the
+ * rows are cut into spans whose partial sums a second pass adds (the same row product as pcgpu_hyrax_open's). */
 int pcgpu_fr_row_mul(pcgpu_ctx *ctx, int curve, const void *v, const void *m, size_t rows, size_t cols, void *out,
                      uint32_t flags);
 
@@ -338,6 +340,46 @@ int pcgpu_mlpc_register(pcgpu_ctx *ctx, int curve, uint32_t nv, const void *cons
 void pcgpu_mlpc_release(pcgpu_ctx *ctx, pcgpu_mlpc *key);
 int pcgpu_mlpc_open(pcgpu_ctx *ctx, const pcgpu_mlpc *key, const void *evals, size_t n, const void *point, uint32_t flags,
                     void *out_proofs_xy, uint8_t *out_proofs_inf, void *out_value);
+
+/* ---- HyraxPC (hyrax/mod.rs) -----------------------------------------------------------------------------------------------
+ * dim = 2^(nv / 2).  Every Fr is Montgomery.  The key (ck / vk) is com_key || h registered with PCGPU_SRS_COMB, dim + 1 bases.
+ * The sponge and the RNG stay with the caller: randomness is an input in the order the reference draws it, challenges in the
+ * order its sponge squeezes them, so the same streams give the reference's proofs byte for byte.
+ * Errors: an odd nv (InvalidNumberOfVariables), a key without comb tables, a key or state of another curve, unknown flags:
+ * PCGPU_E_BADARG; a key that does not hold dim + 1 bases (pedersen_commit's assert_eq) or a state whose nv differs from the
+ * point's (MismatchedNumVars): PCGPU_E_LEN; an input Fr not below r: PCGPU_E_RANGE.  nv = 0 (dim = 1, l = r = [1]) is valid.
+ * Flags: PCGPU_DEVICE_PTRS makes the arguments each call names device pointers; every other argument is a host pointer.
+ * Profile stage 19 (transpose, tensors, row product, inner products); the comb rows are stage 10, the small MSMs stage 4.
+ *
+ * pcgpu_hyrax_commit: HyraxPC::commit of one polynomial (:213-252).  evals: 2^nv elements in to_evaluations() order;
+ *   randomness: dim elements, r_i of row i.  The device transposes evals into the dim x (dim + 1) block [T | r]
+ *   (flat_to_matrix_column_major, utils.rs:13-21) and commits to every row over the key: out_row_coms_xy / _inf receive dim
+ *   points (inf may be NULL).  The block stays on the device in *out, the HyraxCommitmentState.  PCGPU_DEVICE_PTRS: evals and
+ *   randomness.
+ * pcgpu_hyrax_release: frees a state once the context's stream is idle.
+ * pcgpu_hyrax_open: everything HyraxPC::open (:273-406) computes before the challenge, for `count` states at one point
+ *   (point: nv elements).  blinds: per polynomial r_eval || d (dim) || r_d || r_b, the reference's draw order (:360, :367-368,
+ *   :373, :377).  With l, r the tensors of the reversed, split point (:299-307), [lt | r_lt] = l^T [T | r], eval = <lt, r>,
+ *   b = <r, d>, and com_eval = [eval, 0.., r_eval], com_d = [d | r_d], com_b = [b, 0.., r_b] as comb rows over the key.
+ *   out_coms_xy / _inf: 3 * count points, per polynomial com_eval, com_d, com_b (the sponge's absorb order; inf may be NULL);
+ *   out_lt: per polynomial lt || r_lt (dim + 1 elements); out_eval: count elements or NULL.  The caller squeezes c and finishes
+ *   with pcgpu_fr_axpy: z = d + c lt; then z_d = c r_lt + r_d and z_b = c r_eval + r_b.  PCGPU_DEVICE_PTRS: blinds and out_lt.
+ * pcgpu_hyrax_check: HyraxPC::check (:418-511) of `count` proofs at one point.  row_coms: count x dim points (inf may be NULL);
+ *   proof_xy / proof_inf: count x 3 points com_eval, com_d, com_b (inf may be NULL); proof_scalars: count x (dim + 2) elements
+ *   z || z_d || z_b; challenges: count elements.  out_ok[j] = 1 exactly when both of the reference's equations hold for proof j,
+ *   each side compared as affine bytes with its infinity flag: (14) com_key[0] <r, z> + h z_b == c com_eval + com_b and
+ *   (13) pedersen(z) + h z_d == c t_prime + com_d, t_prime = msm(row_coms, l).  The reference's answer is the AND of out_ok.
+ *   Returns PCGPU_OK whether or not the proofs verify.  PCGPU_DEVICE_PTRS: row_coms_xy, row_coms_inf and proof_scalars. */
+typedef struct pcgpu_hyrax pcgpu_hyrax;
+int pcgpu_hyrax_commit(pcgpu_ctx *ctx, const pcgpu_srs *ck, uint32_t nv, const void *evals, const void *randomness, uint32_t flags,
+                       void *out_row_coms_xy, uint8_t *out_row_coms_inf, pcgpu_hyrax **out);
+void pcgpu_hyrax_release(pcgpu_ctx *ctx, pcgpu_hyrax *state);
+int pcgpu_hyrax_open(pcgpu_ctx *ctx, const pcgpu_srs *ck, const pcgpu_hyrax *const *states, size_t count, uint32_t nv,
+                     const void *point, const void *blinds, uint32_t flags, void *out_coms_xy, uint8_t *out_coms_inf, void *out_lt,
+                     void *out_eval);
+int pcgpu_hyrax_check(pcgpu_ctx *ctx, const pcgpu_srs *vk, uint32_t nv, size_t count, const void *row_coms_xy,
+                      const uint8_t *row_coms_inf, const void *point, const void *proof_xy, const uint8_t *proof_inf,
+                      const void *proof_scalars, const void *challenges, uint32_t flags, uint8_t *out_ok);
 
 /* ---- pairing (verifiers) ----------------------------------------------------------------------------------------------
  * E::multi_pairing(a, b) for `count` independent equations of k pairs each: equation j is

@@ -7,9 +7,9 @@ the reference's operator interface for the path (``kzg10.KZG10.commit/open``, ``
 There is no CPU fallback: importing works anywhere, but creating an ``Engine`` raises unless the CUDA
 library is present AND an sm_90 device is usable.
 """
-from .binding import (Engine, Srs, BrakedownCode, MlpcKey, G2Prepared, PcgpuError, CURVES, BLS12_381, BN254, PALLAS, BLS12_381_G2, BN254_G2,
+from .binding import (Engine, Srs, BrakedownCode, MlpcKey, G2Prepared, HyraxState, PcgpuError, CURVES, BLS12_381, BN254, PALLAS, BLS12_381_G2, BN254_G2,
                       SCALARS_MONT, DEVICE_PTRS, SRS_PRECOMPUTE, NTT_INVERSE, SRS_COMB, library_path, fq_limbs, affine_limbs)
 
-__all__ = ["Engine", "Srs", "BrakedownCode", "MlpcKey", "G2Prepared", "PcgpuError", "CURVES", "BLS12_381", "BN254", "PALLAS", "BLS12_381_G2",
+__all__ = ["Engine", "Srs", "BrakedownCode", "MlpcKey", "G2Prepared", "HyraxState", "PcgpuError", "CURVES", "BLS12_381", "BN254", "PALLAS", "BLS12_381_G2",
            "BN254_G2", "SCALARS_MONT", "DEVICE_PTRS", "SRS_PRECOMPUTE", "NTT_INVERSE", "SRS_COMB", "library_path", "fq_limbs",
            "affine_limbs"]

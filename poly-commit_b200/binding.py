@@ -105,6 +105,10 @@ def _load(path):
         "pcgpu_g2_prepare": [_vp, ctypes.c_int, _vp, _vp, _sz, ctypes.c_uint32, ctypes.POINTER(_vp)],
         "pcgpu_g2_prepared_release": [_vp, _vp],
         "pcgpu_multi_pairing_prepared": [_vp, ctypes.c_int, _vp, _vp, _vp, _vp, _sz, _sz, ctypes.c_uint32, _vp, _vp],
+        "pcgpu_hyrax_commit": [_vp, _vp, ctypes.c_uint32, _vp, _vp, ctypes.c_uint32, _vp, _vp, ctypes.POINTER(_vp)],
+        "pcgpu_hyrax_release": [_vp, _vp],
+        "pcgpu_hyrax_open": [_vp, _vp, ctypes.POINTER(_vp), _sz, ctypes.c_uint32, _vp, _vp, ctypes.c_uint32, _vp, _vp, _vp, _vp],
+        "pcgpu_hyrax_check": [_vp, _vp, ctypes.c_uint32, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_uint32, _vp],
         "pcgpu_ipa_begin": [_vp, ctypes.c_int, _vp, _sz, _vp, _sz, _vp, ctypes.c_uint32, ctypes.POINTER(_vp)],
         "pcgpu_ipa_round_lr": [_vp, _vp, _vp, _vp, _vp, _vp, _vp],
         "pcgpu_ipa_round_fold": [_vp, _vp, _vp, _vp],
@@ -154,7 +158,7 @@ def _load(path):
             continue
         fn.argtypes = args
         fn.restype = None if name in ("pcgpu_destroy", "pcgpu_srs_release", "pcgpu_brakedown_release", "pcgpu_mlpc_release",
-                                      "pcgpu_g2_prepared_release") else ctypes.c_int
+                                      "pcgpu_g2_prepared_release", "pcgpu_hyrax_release") else ctypes.c_int
     return lib
 
 
@@ -242,6 +246,16 @@ class G2Prepared(_Handle):
 
     def _free(self, h, ctx):
         self.engine.lib.pcgpu_g2_prepared_release(ctx, h)
+
+
+class HyraxState(_Handle):
+    """Device-resident HyraxCommitmentState of one polynomial: the dim x (dim + 1) block [T | r] its commitment was made from."""
+
+    def __init__(self, engine, handle, curve, nv):
+        self.engine, self.handle, self.curve, self.nv = engine, handle, curve, nv
+
+    def _free(self, h, ctx):
+        self.engine.lib.pcgpu_hyrax_release(ctx, h)
 
 
 class DeviceBuffer(_Handle):
@@ -475,6 +489,50 @@ class Engine:
             out = np.zeros((n, affine_limbs(group)), dtype=np.uint64)
         self._ck(self.lib.pcgpu_g2_fixed_base_mul(self.ctx, group, _ptr(base_xy), _ptr(scalars), n, flags, _ptr(out)))
         return out
+
+    # ---- HyraxPC ----
+    def hyrax_commit(self, ck, nv, evals, randomness, flags=0):
+        """HyraxPC::commit of one polynomial over the comb key ck (com_key || h): evals (2^nv, 4) and randomness (dim, 4)
+        Montgomery Fr, or device pointers with DEVICE_PTRS -> (row_coms (dim, 2*limbs) uint64, identity flags (dim,) uint8,
+        HyraxState)"""
+        evals, randomness = _u64(evals), _u64(randomness)
+        dim = 1 << (nv // 2)
+        out = np.zeros((dim, 2 * fq_limbs(ck.curve)), dtype=np.uint64)
+        inf = np.zeros(dim, dtype=np.uint8)
+        h = _vp()
+        self._ck(self.lib.pcgpu_hyrax_commit(self.ctx, ck.handle, nv, _ptr(evals), _ptr(randomness), flags, _ptr(out), _ptr(inf),
+                                             ctypes.byref(h)))
+        return out, inf, HyraxState(self, h, ck.curve, nv)
+
+    def hyrax_open(self, ck, states, point, blinds, nv=None, flags=0, out_lt=None):
+        """HyraxPC::open up to the challenge for the states at one point (nv, 4); blinds: per state r_eval || d || r_d || r_b
+        ((count * (dim + 3), 4), or a device pointer with DEVICE_PTRS, when out_lt must be a device pointer too) ->
+        (coms (count, 3, 2*limbs): com_eval, com_d, com_b; identity flags (count, 3); lt || r_lt (count, dim + 1, 4) or out_lt;
+        eval (count, 4))"""
+        point, blinds = _u64(point), _u64(blinds)
+        nv = point.size // 4 if nv is None else nv
+        count, dim = len(states), 1 << (nv // 2)
+        hs = (_vp * max(count, 1))(*[s.handle for s in states])
+        coms = np.zeros((count, 3, 2 * fq_limbs(ck.curve)), dtype=np.uint64)
+        inf = np.zeros((count, 3), dtype=np.uint8)
+        lt = np.zeros((count, dim + 1, 4), dtype=np.uint64) if out_lt is None else out_lt
+        ev = np.zeros((count, 4), dtype=np.uint64)
+        self._ck(self.lib.pcgpu_hyrax_open(self.ctx, ck.handle, hs, count, nv, _ptr(point), _ptr(blinds), flags, _ptr(coms), _ptr(inf),
+                                           _ptr(lt), _ptr(ev)))
+        return coms, inf, lt, ev
+
+    def hyrax_check(self, vk, nv, count, row_coms, point, proof_xy, proof_scalars, challenges, row_coms_inf=None, proof_inf=None,
+                    flags=0):
+        """HyraxPC::check of count proofs at one point: row_coms (count * dim, 2*limbs), proof_xy (count * 3, 2*limbs) com_eval,
+        com_d, com_b, proof_scalars (count * (dim + 2), 4) z || z_d || z_b, challenges (count, 4); row_coms, row_coms_inf and
+        proof_scalars are device pointers with DEVICE_PTRS -> (count,) bool"""
+        row_coms, point, proof_xy, proof_scalars, challenges = (_u64(a) for a in (row_coms, point, proof_xy, proof_scalars, challenges))
+        row_coms_inf, proof_inf = (f if f is None or isinstance(f, (int, np.integer)) else np.ascontiguousarray(f, dtype=np.uint8)
+                                   for f in (row_coms_inf, proof_inf))
+        ok = np.zeros(max(count, 1), dtype=np.uint8)
+        self._ck(self.lib.pcgpu_hyrax_check(self.ctx, vk.handle, nv, count, _ptr(row_coms), _ptr(row_coms_inf), _ptr(point),
+                                            _ptr(proof_xy), _ptr(proof_inf), _ptr(proof_scalars), _ptr(challenges), flags, _ptr(ok)))
+        return ok[:count].astype(bool)
 
     # ---- MultilinearPC ----
     def mlpc_register(self, curve, powers_of_h, inf=None, flags=0):

@@ -35,6 +35,7 @@ static void free_device(pcgpu_mlpc *key) { free_device(&key->key); }
 static void free_device(pcgpu_brakedown *code) { rt::dev_free(code->d_mem); }
 static void free_device(pcgpu_ipa *) {}
 static void free_device(pcgpu_g2_prepared *q) { rt::dev_free(q->d_lines); }
+static void free_device(pcgpu_hyrax *h) { rt::dev_free(h->d_block); }
 
 // Every creating entry point: *out is cleared whenever out is non-null, then make(handle) fills a fresh handle under the
 // context's lock.  *out receives the handle only when make succeeds; on failure its device memory is freed and it is deleted.
@@ -367,6 +368,44 @@ extern "C" int pcgpu_msm_batch(pcgpu_ctx *ctx, const pcgpu_srs *srs, const void 
                                void *out_xy, uint8_t *out_inf) {
   return on_ctx(ctx, !srs || (n && count && !scalars) || (count && !out_xy), [&]() -> int {
     DISPATCH_CURVE(srs->curve, return msm_batch_impl<C>(ctx, srs, scalars, n, count, flags, out_xy, out_inf));
+  });
+}
+
+// ---- HyraxPC (hyrax.cuh) -------------------------------------------------------------------------------------------------
+// an odd number of variables is InvalidNumberOfVariables (hyrax/mod.rs:220-224, :289-293, :432-436); nv > 52 cannot be addressed
+static bool hyrax_nv_bad(uint32_t nv) { return (nv & 1) || nv > 52; }
+
+extern "C" int pcgpu_hyrax_commit(pcgpu_ctx *ctx, const pcgpu_srs *ck, uint32_t nv, const void *evals, const void *randomness,
+                                  uint32_t flags, void *out_row_coms_xy, uint8_t *out_row_coms_inf, pcgpu_hyrax **out) {
+  const bool bad_args = !ck || !evals || !randomness || !out_row_coms_xy || hyrax_nv_bad(nv) || (flags & ~(uint32_t)PCGPU_DEVICE_PTRS);
+  return create(ctx, bad_args, out, [&](pcgpu_hyrax *h) -> int {
+    DISPATCH_CURVE(ck->curve, return hyrax_commit_impl<C>(ctx, ck, nv, evals, randomness, flags, out_row_coms_xy, out_row_coms_inf, h));
+  });
+}
+
+extern "C" void pcgpu_hyrax_release(pcgpu_ctx *ctx, pcgpu_hyrax *state) { release_after_stream(ctx, state); }
+
+extern "C" int pcgpu_hyrax_open(pcgpu_ctx *ctx, const pcgpu_srs *ck, const pcgpu_hyrax *const *states, size_t count, uint32_t nv,
+                                const void *point, const void *blinds, uint32_t flags, void *out_coms_xy, uint8_t *out_coms_inf,
+                                void *out_lt, void *out_eval) {
+  bool bad_args = !ck || hyrax_nv_bad(nv) || (nv && !point) || (count && (!states || !blinds || !out_coms_xy || !out_lt)) ||
+                  (flags & ~(uint32_t)PCGPU_DEVICE_PTRS);
+  for (size_t p = 0; !bad_args && p < count; p++) bad_args = !states[p];
+  return on_ctx(ctx, bad_args, [&]() -> int {
+    DISPATCH_CURVE(ck->curve, return hyrax_open_impl<C>(ctx, ck, states, count, nv, point, blinds, flags, out_coms_xy, out_coms_inf,
+                                                        out_lt, out_eval));
+  });
+}
+
+extern "C" int pcgpu_hyrax_check(pcgpu_ctx *ctx, const pcgpu_srs *vk, uint32_t nv, size_t count, const void *row_coms_xy,
+                                 const uint8_t *row_coms_inf, const void *point, const void *proof_xy, const uint8_t *proof_inf,
+                                 const void *proof_scalars, const void *challenges, uint32_t flags, uint8_t *out_ok) {
+  const bool bad_args = !vk || hyrax_nv_bad(nv) || (nv && !point) ||
+                        (count && (!row_coms_xy || !proof_xy || !proof_scalars || !challenges || !out_ok)) ||
+                        (flags & ~(uint32_t)PCGPU_DEVICE_PTRS);
+  return on_ctx(ctx, bad_args, [&]() -> int {
+    DISPATCH_CURVE(vk->curve, return hyrax_check_impl<C>(ctx, vk, nv, count, row_coms_xy, row_coms_inf, point, proof_xy, proof_inf,
+                                                         proof_scalars, challenges, flags, out_ok));
   });
 }
 

@@ -500,17 +500,74 @@ inline int fr_inner_product(const uint32_t *a, const uint32_t *b, size_t n, uint
   return rt::launch_blocks<IP_BLOCK>(FrBlockSumBody<R>{lvl1, nblk, out, (uint32_t)nblk}, 1, IP_BLOCK * 32, st);
 }
 
-// out[c] = sum_r v[r] * M[r*cols + c]   (thread per column; coalesced across columns)
+// ---------------------------------------------------------------------------------------------
+// row product  out_p[c] = sum_r v[r] * M_p[r*cols + c]  for `count` matrices M_p of rows x cols (Matrix::row_mul, utils.rs:127-146)
+// One thread per (matrix, row span, column): coalesced across columns.  When the columns alone cannot fill the device (Hyrax's
+// 2^11 x (2^11 + 1) block at cfg4 is 2049 threads) the rows are cut into `splits` spans whose partial sums a second pass adds.
+// ---------------------------------------------------------------------------------------------
+enum { ROWMUL_THREADS = 1 << 17, ROWMUL_MIN_SPAN = 16, ROWMUL_MAX_SPLITS = 1024 };
+struct RowMulPlan {
+  size_t rows, cols, count;
+  uint32_t splits;   // row spans per matrix (1: one pass straight into out)
+  size_t span;       // rows per span
+  size_t partial;    // Fr elements of partial-sum scratch (0 when splits == 1)
+};
+// the fewest spans (a power of two) that give ROWMUL_THREADS threads, while every span keeps >= ROWMUL_MIN_SPAN rows
+inline RowMulPlan row_mul_plan(size_t rows, size_t cols, size_t count) {
+  RowMulPlan p{rows, cols, count, 1, rows, 0};
+  while (p.splits < ROWMUL_MAX_SPLITS && count * cols * p.splits < (size_t)ROWMUL_THREADS && rows / (2 * (size_t)p.splits) >= ROWMUL_MIN_SPAN)
+    p.splits *= 2;
+  p.span = (rows + p.splits - 1) / p.splits;
+  if (p.splits > 1) p.partial = count * cols * p.splits;
+  return p;
+}
+
 template <class R>
 struct FrRowMulBody {
-  const uint32_t *v; const uint32_t *m; size_t rows, cols; uint32_t *out;
-  PCGPU_KERNEL_DEV void operator()(size_t c) const {
+  const uint32_t *v; const uint32_t *const *mats; RowMulPlan p; uint32_t *out; size_t out_stride; uint32_t *partial;
+  PCGPU_KERNEL_DEV void operator()(size_t t) const {
+    const size_t c = t % p.cols, s = (t / p.cols) % p.splits, q = t / (p.cols * p.splits);
+    const uint32_t *m = mats[q];
+    const size_t r0 = s * p.span, r1 = r0 + p.span < p.rows ? r0 + p.span : p.rows;
     Fp<R> acc = Fp<R>::zero();
-    size_t r = 0;
-    for (; r + 2 <= rows; r += 2)      // pairs of rows: one reduction per two products (fr_dot2)
-      acc = fp_add<R>(acc, fr_dot2<R>(load_fr<R>(v, r), load_fr<R>(m, r * cols + c), load_fr<R>(v, r + 1), load_fr<R>(m, (r + 1) * cols + c)));
-    if (r < rows) acc = fp_add<R>(acc, fp_mul<R>(load_fr<R>(v, r), load_fr<R>(m, r * cols + c)));
-    store_fr<R>(out, c, acc);
+    size_t r = r0;
+    for (; r + 2 <= r1; r += 2)      // pairs of rows: one reduction per two products (fr_dot2)
+      acc = fp_add<R>(acc, fr_dot2<R>(load_fr<R>(v, r), load_fr<R>(m, r * p.cols + c), load_fr<R>(v, r + 1), load_fr<R>(m, (r + 1) * p.cols + c)));
+    if (r < r1) acc = fp_add<R>(acc, fp_mul<R>(load_fr<R>(v, r), load_fr<R>(m, r * p.cols + c)));
+    if (p.splits == 1) store_fr<R>(out, q * out_stride + c, acc);
+    else store_fr<R>(partial, t, acc);
+  }
+};
+template <class R>
+struct FrRowMulSumBody {
+  const uint32_t *partial; RowMulPlan p; uint32_t *out; size_t out_stride;
+  PCGPU_KERNEL_DEV void operator()(size_t t) const {
+    const size_t c = t % p.cols, q = t / p.cols;
+    Fp<R> acc = Fp<R>::zero();
+    for (uint32_t s = 0; s < p.splits; s++) acc = fp_add<R>(acc, load_fr<R>(partial, (q * p.splits + s) * p.cols + c));
+    store_fr<R>(out, q * out_stride + c, acc);
+  }
+};
+// v: p.rows elements; mats: device array of p.count device pointers; out: matrix q's row product at out + q * out_stride elements;
+// partial: p.partial elements of scratch
+template <class R>
+inline int fr_row_mul_run(const RowMulPlan &p, const uint32_t *v, const uint32_t *const *mats, uint32_t *out, size_t out_stride,
+                          uint32_t *partial, rt::stream_t st) {
+  int rc;
+  if ((rc = rt::launch<128>(FrRowMulBody<R>{v, mats, p, out, out_stride, partial}, p.count * p.cols * p.splits, st))) return rc;
+  if (p.splits == 1) return rt::OK;
+  return rt::launch<128>(FrRowMulSumBody<R>{partial, p, out, out_stride}, p.count * p.cols, st);
+}
+
+// err |= 1 when an element of v (n Montgomery or canonical Fr, as stored) is not below r
+template <class R>
+struct FrBelowModulusBody {
+  const uint32_t *v; uint32_t *err;
+  PCGPU_KERNEL_DEV void operator()(size_t i) const {
+    const Fp<R> s = load_fr<R>(v, i);
+    bool lt_r = false, decided = false;
+    for (int j = 7; j >= 0; j--) if (!decided && s.l[j] != R::mod(j)) { lt_r = s.l[j] < R::mod(j); decided = true; }
+    if (!lt_r) rt::atomic_or(err, 1u);
   }
 };
 

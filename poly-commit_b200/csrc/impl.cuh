@@ -6,6 +6,7 @@
 // the kernel bodies serially; the package never loads that library.
 #pragma once
 #include <algorithm>
+#include <initializer_list>
 #include <memory>
 #include <mutex>
 #include <new>
@@ -29,13 +30,14 @@
 #include "field_ops.cuh"
 #include "mlpc.cuh"
 #include "pairing.cuh"
+#include "hyrax.cuh"
 
 using namespace pcgpu;
 
 // ---------------------------------------------------------------------------------------------
 // profiling (CUDA events on the launching stream)
 // ---------------------------------------------------------------------------------------------
-enum { PROF_STAGES = 19 };
+enum { PROF_STAGES = 20 };
 struct Prof {
   bool on = false;
   double ms[PROF_STAGES] = {0};
@@ -98,6 +100,7 @@ struct DeviceWords {
   uint32_t peer_timeout;             // PeerWaitBody: non-zero when a peer missed the deadline
   unsigned long long last_nonzero;   // FrLastNonzeroBody: one past the last non-zero coefficient
   uint32_t selftest_bad;             // FieldSelfTestBody: mismatch count
+  uint32_t range_err;                // FrBelowModulusBody: an input element not below r
 };
 
 struct pcgpu_ctx {
@@ -304,7 +307,7 @@ int srs_register_impl(pcgpu_ctx *ctx, const void *bases, const uint8_t *inf, siz
 // ---------------------------------------------------------------------------------------------
 // helpers
 // ---------------------------------------------------------------------------------------------
-// Small MSMs (msm_small.cuh): up to SMALL_MAX_PROB problems of <= SMALL_MAX_N terms in one launch; one point per window
+// Small MSMs (msm_small.cuh): up to SMALL_MAX_PROB problems of <= 2 SMALL_MAX_N terms in one launch; one point per window
 // comes back and the host finishes with the doublings.  PCGPU_MSM_SMALL=0 forces the bucket pipeline (tests, A/B timing).
 inline bool msm_small_enabled() {
   const char *e = getenv("PCGPU_MSM_SMALL");
@@ -392,12 +395,13 @@ int msm_small_to_host(pcgpu_ctx *ctx, const MsmPlan &p, const MsmSmallProblem<C>
   msm_report(ctx, p);
   const uint32_t split = p.split;   // blocks per window
   const size_t npts = (size_t)nprob * W * split;
-  uint32_t *d_err; XYZZ<C> *d_out;
-  if ((rc = ctx->msm_arena.carve([&](auto &&buf) { buf(d_err, 1); buf(d_out, npts); }))) return rc;
+  uint32_t *d_err; XYZZ<C> *d_out; MsmSmallProblem<C> *d_prob;
+  if ((rc = ctx->msm_arena.carve([&](auto &&buf) { buf(d_err, 1); buf(d_out, npts); buf(d_prob, nprob); }))) return rc;
   if ((rc = rt::dev_memset(d_err, 0, sizeof *d_err, st))) return rc;
+  if ((rc = rt::copy_h2d(d_prob, probs, nprob * sizeof *probs, st))) return rc;
   MsmSmallBody<C> body;
   memset(&body, 0, sizeof body);
-  for (uint32_t p = 0; p < nprob; p++) body.prob[p] = probs[p];
+  body.prob = d_prob;
   body.mont = mont ? 1u : 0u; body.split = split; body.out = d_out; body.err = d_err;
   ctx->prof.begin(4, st);
   if ((rc = rt::launch_blocks<SMALL_BLOCK>(body, npts, msm_small_smem<C>(), st))) return rc;
@@ -614,12 +618,63 @@ int g1_sum_impl(pcgpu_ctx *, const void *xyzz, size_t count, void *out_xy, uint8
   return PCGPU_OK;
 }
 
+// `count` comb rows over srs's PCGPU_SRS_COMB tables, left on the device: d_out[r] = sum_i d_s[r*n + i] * bases[i] (affine, the
+// identity as Affine::inf()).  The accumulate scratch comes from the context's MSM arena; *d_err (in that arena) is non-zero
+// when a scalar was not a reduced field element.  Profile stage 10.  The one comb launch sequence: pcgpu_msm_batch and the
+// Hyrax commit, open and check all run their rows here.
+template <class C>
+int comb_rows(pcgpu_ctx *ctx, const pcgpu_srs *srs, const uint32_t *d_s, size_t n, size_t count, bool mont, Affine<C> *d_out,
+              uint32_t **d_err) {
+  rt::stream_t st = ctx->stream;
+  int rc;
+  CombGeom g = comb_geometry<C>(srs->n, srs->comb_c);
+  g.n = (uint32_t)n; g.count = (uint32_t)count;
+  g.seg_len = 64; if (count < 4096) { while (g.seg_len > 8 && count * ((n + g.seg_len - 1) / g.seg_len) < 65536) g.seg_len /= 2; }
+  g.segs = (uint32_t)((n + g.seg_len - 1) / g.seg_len);
+  g.scalar_bits = C::Fr::BITS; g.scalars_mont = mont ? 1 : 0;
+  const size_t ntasks = count * g.segs;
+  comb_report(ctx, g);
+  XYZZ<C> *partial;
+  if ((rc = ctx->msm_arena.carve([&](auto &&buf) { buf(*d_err, 16); buf(partial, ntasks); }))) return rc;
+  if ((rc = rt::dev_memset(*d_err, 0, 64, st))) return rc;
+  if ((rc = ensure_pow2<C>(ctx))) return rc;
+  ctx->prof.begin(10, st);
+  if ((rc = rt::launch<128>(CombAccumulateBody<C>{(const Affine<C> *)srs->d_comb, d_s, g, partial, *d_err}, ntasks, st))) return rc;
+  if ((rc = rt::launch<64>(CombRowSumBody<C>{partial, g.segs, d_out, ctx->d_pow2[C::ID]}, count, st))) return rc;
+  ctx->prof.end(10, st);
+  return PCGPU_OK;
+}
+
+// `count` device affine points -> the caller's x || y and infinity bytes (out_inf may be NULL); waits for the stream
+template <class C>
+int affine_to_host(pcgpu_ctx *ctx, const Affine<C> *d_pts, size_t count, void *out_xy, uint8_t *out_inf) {
+  const size_t psz = sizeof(Affine<C>);
+  std::vector<Affine<C>> h(count);
+  int rc;
+  if ((rc = rt::copy_d2h(h.data(), d_pts, count * psz, ctx->stream))) return rc;
+  if ((rc = rt::stream_sync(ctx->stream))) return rc;
+  for (size_t r = 0; r < count; r++) {
+    bool inf = h[r].is_inf();
+    memcpy((char *)out_xy + r * psz, &h[r], psz);
+    if (out_inf) out_inf[r] = inf ? 1 : 0;
+  }
+  return PCGPU_OK;
+}
+
+// the context's error word after the stream drained: PCGPU_E_RANGE when set
+inline int read_err_word(pcgpu_ctx *ctx, const uint32_t *d_err) {
+  uint32_t h = 0;
+  int rc;
+  if ((rc = rt::copy_d2h(&h, d_err, 4, ctx->stream)) || (rc = rt::stream_sync(ctx->stream))) return rc;
+  ctx->prof.collect();
+  return h ? PCGPU_E_RANGE : PCGPU_OK;
+}
+
 // `count` MSMs over shared bases (hyrax/mod.rs:233-242)
 template <class C>
 int msm_batch_impl(pcgpu_ctx *ctx, const pcgpu_srs *srs, const void *scalars, size_t n, size_t count, uint32_t flags,
                    void *out_xy, uint8_t *out_inf) {
   if (n > srs->n) return PCGPU_E_LEN;
-  rt::stream_t st = ctx->stream;
   int rc;
   const size_t psz = sizeof(Affine<C>);
   const bool mont = (flags & PCGPU_SCALARS_MONT) != 0;
@@ -632,37 +687,196 @@ int msm_batch_impl(pcgpu_ctx *ctx, const pcgpu_srs *srs, const void *scalars, si
     }
     return PCGPU_OK;
   }
-  CombGeom g = comb_geometry<C>(srs->n, srs->comb_c);
-  g.n = (uint32_t)n; g.count = (uint32_t)count;
-  g.seg_len = 64; if (count < 4096) { while (g.seg_len > 8 && count * ((n + g.seg_len - 1) / g.seg_len) < 65536) g.seg_len /= 2; }
-  g.segs = (uint32_t)((n + g.seg_len - 1) / g.seg_len);
-  g.scalar_bits = C::Fr::BITS; g.scalars_mont = mont ? 1 : 0;
-  size_t ntasks = count * g.segs;
-  comb_report(ctx, g);
-  uint32_t *d_err; XYZZ<C> *partial; Affine<C> *d_out; const uint32_t *d_s;
+  Affine<C> *d_out; const uint32_t *d_s; uint32_t *d_err;
   Staging io(ctx, flags);
-  io.scratch(d_err, 64);
-  io.scratch(partial, ntasks * sizeof(XYZZ<C>));
   io.scratch(d_out, count * psz);
   io.in(d_s, scalars, count * n * 32);
   if ((rc = io.upload())) return rc;
-  if ((rc = rt::dev_memset(d_err, 0, 64, st))) return rc;
-  ctx->prof.begin(10, st);
-  if ((rc = rt::launch<128>(CombAccumulateBody<C>{(const Affine<C> *)srs->d_comb, d_s, g, partial, d_err}, ntasks, st))) return rc;
-  if ((rc = ensure_pow2<C>(ctx))) return rc;
-  if ((rc = rt::launch<64>(CombRowSumBody<C>{partial, g.segs, d_out, ctx->d_pow2[C::ID]}, count, st))) return rc;
-  ctx->prof.end(10, st);
-  std::vector<Affine<C>> h(count);
-  uint32_t herr = 0;
-  if ((rc = rt::copy_d2h(h.data(), d_out, count * psz, st))) return rc;
-  if ((rc = rt::copy_d2h(&herr, d_err, 4, st))) return rc;
-  if ((rc = rt::stream_sync(st))) return rc;
-  ctx->prof.collect();
-  if (herr) return PCGPU_E_RANGE;
-  for (size_t r = 0; r < count; r++) {
-    bool inf = h[r].is_inf();
-    memcpy((char *)out_xy + r * psz, &h[r], psz);
-    if (out_inf) out_inf[r] = inf ? 1 : 0;
+  if ((rc = comb_rows<C>(ctx, srs, d_s, n, count, mont, d_out, &d_err))) return rc;
+  if ((rc = read_err_word(ctx, d_err))) return rc;
+  return affine_to_host<C>(ctx, d_out, count, out_xy, out_inf);
+}
+
+// ---------------------------------------------------------------------------------------------
+// HyraxPC (hyrax.cuh): the resident commitment state, the dot-product opening before the challenge, and check
+// ---------------------------------------------------------------------------------------------
+// HyraxCommitmentState (hyrax/data_structures.rs): the dim x (dim + 1) block [T | r], row-major, resident on the device
+struct pcgpu_hyrax {
+  int curve = 0;
+  uint32_t nv = 0;
+  size_t dim = 0;
+  uint32_t *d_block = nullptr;
+};
+
+// PCGPU_E_RANGE when an element of any of the (device pointer, count) arrays is not below r; waits for the stream
+template <class C>
+int fr_range_check(pcgpu_ctx *ctx, std::initializer_list<std::pair<const uint32_t *, size_t>> arrays) {
+  rt::stream_t st = ctx->stream;
+  uint32_t *d_err = &ctx->d_words->range_err;
+  int rc;
+  if ((rc = rt::dev_memset(d_err, 0, 4, st))) return rc;
+  for (const auto &a : arrays)
+    if ((rc = rt::launch<256>(FrBelowModulusBody<typename C::Fr>{a.first, d_err}, a.second, st))) return rc;
+  return read_err_word(ctx, d_err);
+}
+
+// the key every Hyrax call runs its comb rows over: com_key || h with comb tables, dim + 1 bases (pedersen_commit's assert_eq)
+inline int hyrax_key_check(const pcgpu_srs *ck, size_t dim) {
+  if (!ck->d_comb) return PCGPU_E_BADARG;
+  return ck->n == dim + 1 ? PCGPU_OK : PCGPU_E_LEN;
+}
+
+// HyraxPC::commit for one polynomial (hyrax/mod.rs:213-252)
+template <class C>
+int hyrax_commit_impl(pcgpu_ctx *ctx, const pcgpu_srs *ck, uint32_t nv, const void *evals, const void *randomness, uint32_t flags,
+                      void *out_xy, uint8_t *out_inf, pcgpu_hyrax *h) {
+  const size_t dim = (size_t)1 << (nv / 2), w = dim + 1;
+  int rc;
+  if ((rc = hyrax_key_check(ck, dim))) return rc;
+  rt::stream_t st = ctx->stream;
+  h->curve = C::ID; h->nv = nv; h->dim = dim;
+  if ((rc = rt::dev_malloc((void **)&h->d_block, dim * w * 32))) return rc;
+  const uint32_t *d_ev, *d_r; Affine<C> *d_out; uint32_t *d_err;
+  Staging io(ctx, flags);
+  io.in(d_ev, evals, dim * dim * 32);
+  io.in(d_r, randomness, dim * 32);
+  io.scratch(d_out, dim * sizeof(Affine<C>));
+  if ((rc = io.upload())) return rc;
+  if ((rc = fr_range_check<C>(ctx, {{d_ev, dim * dim}, {d_r, dim}}))) return rc;
+  const uint32_t tiles = (uint32_t)((dim + HYRAX_TILE - 1) / HYRAX_TILE);
+  ctx->prof.begin(19, st);
+  if ((rc = rt::launch_blocks<256>(HyraxTransposeBody{d_ev, d_r, h->d_block, (uint32_t)dim, tiles}, (size_t)tiles * tiles,
+                                   hyrax_transpose_smem(), st))) return rc;
+  ctx->prof.end(19, st);
+  if ((rc = comb_rows<C>(ctx, ck, h->d_block, w, dim, true, d_out, &d_err))) return rc;   // mod.rs:233-242
+  if ((rc = read_err_word(ctx, d_err))) return rc;
+  return affine_to_host<C>(ctx, d_out, dim, out_xy, out_inf);
+}
+
+// HyraxPC::open up to the challenge (hyrax/mod.rs:273-390) for `count` states at one point
+template <class C>
+int hyrax_open_impl(pcgpu_ctx *ctx, const pcgpu_srs *ck, const pcgpu_hyrax *const *states, size_t count, uint32_t nv,
+                    const void *point, const void *blinds, uint32_t flags, void *out_coms_xy, uint8_t *out_coms_inf, void *out_lt,
+                    void *out_eval) {
+  using R = typename C::Fr;
+  const size_t dim = (size_t)1 << (nv / 2), w = dim + 1;
+  int rc;
+  if ((rc = hyrax_key_check(ck, dim))) return rc;
+  for (size_t p = 0; p < count; p++) {
+    if (states[p]->curve != C::ID) return PCGPU_E_BADARG;
+    if (states[p]->nv != nv) return PCGPU_E_LEN;                    // MismatchedNumVars, mod.rs:328-333
+  }
+  if (count == 0) return PCGPU_OK;
+  rt::stream_t st = ctx->stream;
+  const RowMulPlan plan = row_mul_plan(dim, w, count);
+  const uint32_t *d_point, *d_bl; uint32_t *d_lt, *d_fr, *d_eval; const uint32_t **d_mats; Affine<C> *d_out;
+  Staging io(ctx, flags);
+  io.host_in(d_point, point, (size_t)nv * 32);
+  io.in(d_bl, blinds, count * (dim + 3) * 32);
+  io.out(d_lt, out_lt, count * w * 32);
+  io.host_out(d_eval, out_eval, count * 32);
+  io.scratch(d_fr, (2 * dim + 3 * count * w + plan.partial) * 32);   // l || r, the comb rows, the row product's partial sums
+  io.scratch(d_mats, count * sizeof *d_mats);
+  io.scratch(d_out, 3 * count * sizeof(Affine<C>));
+  if ((rc = io.upload())) return rc;
+  uint32_t *d_tensor = d_fr, *d_rows = d_fr + 8 * 2 * dim, *d_partial = d_rows + 8 * 3 * count * w;
+  std::vector<const uint32_t *> mats(count);
+  for (size_t p = 0; p < count; p++) mats[p] = states[p]->d_block;
+  if ((rc = rt::copy_h2d(d_mats, mats.data(), count * sizeof *d_mats, st))) return rc;
+  if ((rc = fr_range_check<C>(ctx, {{d_point, nv}, {d_bl, count * (dim + 3)}}))) return rc;
+  ctx->prof.begin(19, st);
+  if ((rc = rt::launch<128>(HyraxTensorBody<R>{d_point, nv / 2, d_tensor}, 2 * dim, st))) return rc;      // mod.rs:299-307
+  if ((rc = fr_row_mul_run<R>(plan, d_tensor, d_mats, d_lt, w, d_partial, st))) return rc;               // [lt | r_lt], :347-354
+  if ((rc = rt::launch_blocks<HYRAX_BLOCK>(HyraxOpenRowsBody<R>{d_lt, d_tensor, d_bl, d_rows, d_eval, (uint32_t)dim}, count,
+                                           HYRAX_BLOCK * 32, st))) return rc;                              // :356-378
+  ctx->prof.end(19, st);
+  uint32_t *d_err;
+  if ((rc = comb_rows<C>(ctx, ck, d_rows, w, 3 * count, true, d_out, &d_err))) return rc;
+  if ((rc = io.download())) return rc;
+  if ((rc = read_err_word(ctx, d_err))) return rc;
+  return affine_to_host<C>(ctx, d_out, 3 * count, out_coms_xy, out_coms_inf);
+}
+
+// HyraxPC::check (hyrax/mod.rs:418-511) of `count` proofs at one point: out_ok[j] = both equations hold for proof j
+template <class C>
+int hyrax_check_impl(pcgpu_ctx *ctx, const pcgpu_srs *vk, uint32_t nv, size_t count, const void *row_coms_xy, const uint8_t *row_coms_inf,
+                     const void *point, const void *proof_xy, const uint8_t *proof_inf, const void *proof_scalars, const void *challenges,
+                     uint32_t flags, uint8_t *out_ok) {
+  using R = typename C::Fr;
+  const size_t dim = (size_t)1 << (nv / 2), w = dim + 1, psz = sizeof(Affine<C>);
+  int rc;
+  if ((rc = hyrax_key_check(vk, dim))) return rc;
+  if (count == 0) return PCGPU_OK;
+  rt::stream_t st = ctx->stream;
+  const size_t npts = count * dim + 3 * count;   // row commitments, then com_eval, com_d, com_b of every proof
+  Affine<C> *d_pts, *d_lhs; const uint8_t *d_rc_inf = nullptr, *d_pf_inf = nullptr; const uint32_t *d_zs, *d_point, *d_ch;
+  uint32_t *d_fr;
+  Staging io(ctx, flags);
+  io.scratch(d_pts, npts * psz);
+  if (row_coms_inf) io.in(d_rc_inf, row_coms_inf, count * dim);
+  if (proof_inf) io.host_in(d_pf_inf, proof_inf, 3 * count);
+  io.in(d_zs, proof_scalars, count * (dim + 2) * 32);
+  io.host_in(d_point, point, (size_t)nv * 32);
+  io.host_in(d_ch, challenges, count * 32);
+  io.scratch(d_fr, (2 * dim + count * dim + 2 * count * w + 1) * 32);   // l || r, c_j l, the comb rows, the scalar one
+  io.scratch(d_lhs, 2 * count * psz);
+  if ((rc = io.upload())) return rc;
+  uint32_t *d_tensor = d_fr, *d_cl = d_fr + 8 * 2 * dim, *d_rows = d_cl + 8 * count * dim, *d_one = d_rows + 8 * 2 * count * w;
+  Affine<C> *d_proof = d_pts + count * dim;
+  if ((rc = copy_in(d_pts, row_coms_xy, count * dim * psz, flags, st))) return rc;
+  if ((rc = rt::copy_h2d(d_proof, proof_xy, 3 * count * psz, st))) return rc;
+  const uint32_t pw = (uint32_t)(psz / 4);
+  if (d_rc_inf && (rc = rt::launch<256>(SrsZeroIdentityBody{(uint32_t *)d_pts, d_rc_inf, pw}, count * dim, st))) return rc;
+  if (d_pf_inf && (rc = rt::launch<256>(SrsZeroIdentityBody{(uint32_t *)d_proof, d_pf_inf, pw}, 3 * count, st))) return rc;
+  if ((rc = fr_range_check<C>(ctx, {{d_zs, count * (dim + 2)}, {d_point, nv}, {d_ch, count}}))) return rc;
+  ctx->prof.begin(19, st);
+  if ((rc = rt::launch<128>(HyraxTensorBody<R>{d_point, nv / 2, d_tensor}, 2 * dim, st))) return rc;      // mod.rs:440-448
+  if ((rc = rt::launch_blocks<HYRAX_BLOCK>(HyraxCheckRowsBody<R>{d_tensor, d_zs, d_ch, d_rows, d_cl, (uint32_t)dim}, count,
+                                           HYRAX_BLOCK * 32, st))) return rc;
+  if ((rc = rt::launch<32>(FrFillOneBody<R>{d_one}, 1, st))) return rc;
+  ctx->prof.end(19, st);
+  // left-hand sides: com_key[0] <r, z> + h z_b (14) and pedersen(z) + h z_d (13), one comb batch
+  uint32_t *d_err;
+  if ((rc = comb_rows<C>(ctx, vk, d_rows, w, 2 * count, true, d_lhs, &d_err))) return rc;
+  if ((rc = read_err_word(ctx, d_err))) return rc;
+  std::vector<uint8_t> lhs_xy(2 * count * psz), lhs_inf(2 * count);
+  if ((rc = affine_to_host<C>(ctx, d_lhs, 2 * count, lhs_xy.data(), lhs_inf.data()))) return rc;
+  // right-hand sides: c com_eval + com_b (14) and msm(row_coms, c l) + com_d = c t_prime + com_d (13)
+  std::vector<host::HXYZZ<C>> rhs(2 * count);
+  std::vector<MsmSmallProblem<C>> probs;
+  for (size_t j = 0; j < count; j++)
+    probs.push_back({d_proof + 3 * j, d_ch + 8 * j, d_proof + 3 * j + 2, d_one, 1u});
+  const bool small = dim <= 2 * SMALL_MAX_N && msm_small_enabled();
+  if (small)
+    for (size_t j = 0; j < count; j++) probs.push_back({d_pts + j * dim, d_cl + 8 * dim * j, d_proof + 3 * j + 1, d_one, (uint32_t)dim});
+  const MsmPlan plan = msm_small_plan(small ? dim : 1);
+  for (size_t off = 0; off < probs.size(); off += SMALL_MAX_PROB) {   // rhs[i] for problem i: all (14), then all (13)
+    const uint32_t np = (uint32_t)std::min(probs.size() - off, (size_t)SMALL_MAX_PROB);
+    if ((rc = msm_small_to_host<C>(ctx, plan, probs.data() + off, np, true, rhs.data() + off))) return rc;
+  }
+  if (!small) {   // the bucket pipeline, one proof at a time; com_d is added on the host
+    for (size_t j = 0; j < count; j++) {
+      const pcgpu_srs view = srs_view<C>(d_pts + j * dim, dim);
+      host::HXYZZ<C> t;
+      if ((rc = msm_to_host<C>(ctx, &view, 0, d_cl + 8 * dim * j, dim, true, &t))) return rc;
+      Affine<C> cd;
+      if ((rc = rt::copy_d2h(&cd, d_proof + 3 * j + 1, psz, st)) || (rc = rt::stream_sync(st))) return rc;
+      uint64_t one[4] = {1, 0, 0, 0};
+      rhs[count + j] = cd.is_inf() ? t : host::padd<C>(t, host::pmul_affine<C>(&cd, one));
+    }
+  }
+  for (size_t j = 0; j < 2 * count; j++) {
+    std::vector<uint8_t> xy(psz);
+    uint8_t inf = 0;
+    host::to_affine<C>(rhs[j], xy.data(), &inf);
+    const size_t row = j < count ? 2 * j : 2 * (j - count) + 1;   // rhs: all (14) then all (13); lhs rows alternate
+    uint8_t *lxy = lhs_xy.data() + row * psz;
+    if (lhs_inf[row]) memset(lxy, 0, psz);
+    if (inf) memset(xy.data(), 0, psz);
+    const bool eq = inf == lhs_inf[row] && memcmp(xy.data(), lxy, psz) == 0;
+    const size_t k = j < count ? j : j - count;
+    if (j < count) out_ok[k] = eq ? 1 : 0;
+    else out_ok[k] = out_ok[k] && eq ? 1 : 0;
   }
   return PCGPU_OK;
 }
@@ -873,13 +1087,17 @@ int fr_row_mul_impl(pcgpu_ctx *ctx, const void *v, const void *m, size_t rows, s
   rt::stream_t st = ctx->stream;
   int rc;
   if (cols == 0) return PCGPU_OK;
-  const uint32_t *dv, *dm; uint32_t *dout;
+  const RowMulPlan plan = row_mul_plan(rows, cols, 1);
+  const uint32_t *dv, *dm; uint32_t *dout, *partial; const uint32_t **d_mats;
   Staging io(ctx, flags);
   io.in(dv, v, rows * 32);
   io.in(dm, m, rows * cols * 32);
   io.out(dout, out, cols * 32);
+  io.scratch(partial, plan.partial * 32);
+  io.scratch(d_mats, sizeof dm);
   if ((rc = io.upload())) return rc;
-  if ((rc = rt::launch<128>(FrRowMulBody<R>{dv, dm, rows, cols, dout}, cols, st))) return rc;
+  if ((rc = rt::copy_h2d(d_mats, &dm, sizeof dm, st))) return rc;
+  if ((rc = fr_row_mul_run<R>(plan, dv, d_mats, dout, 0, partial, st))) return rc;
   if ((rc = io.download())) return rc;
   return rt::stream_sync(st);
 }
@@ -2041,7 +2259,12 @@ inline int measure_imad_peak_impl(pcgpu_ctx *ctx, double *ops_per_s) {
                                     const void *, size_t, uint32_t, void *, uint8_t *, void *); \
   EXT template int msm_batch_impl<C>(pcgpu_ctx *, const pcgpu_srs *, const void *, size_t, size_t, uint32_t, void *, uint8_t *); \
   EXT template int kzg_commit_open_impl<C>(pcgpu_ctx *, pcgpu_ctx *, const pcgpu_srs *, const void *, size_t, const void *, uint32_t, void *, uint8_t *, void *, uint8_t *); \
-  EXT template int msm_peer_impl<C>(pcgpu_ctx *, const pcgpu_srs *, size_t, const void *, size_t, uint32_t, void *const *, uint32_t, uint32_t, uint64_t, void *, uint8_t *);
+  EXT template int msm_peer_impl<C>(pcgpu_ctx *, const pcgpu_srs *, size_t, const void *, size_t, uint32_t, void *const *, uint32_t, uint32_t, uint64_t, void *, uint8_t *); \
+  EXT template int hyrax_commit_impl<C>(pcgpu_ctx *, const pcgpu_srs *, uint32_t, const void *, const void *, uint32_t, void *, uint8_t *, pcgpu_hyrax *); \
+  EXT template int hyrax_open_impl<C>(pcgpu_ctx *, const pcgpu_srs *, const pcgpu_hyrax *const *, size_t, uint32_t, const void *, const void *, \
+                                      uint32_t, void *, uint8_t *, void *, void *); \
+  EXT template int hyrax_check_impl<C>(pcgpu_ctx *, const pcgpu_srs *, uint32_t, size_t, const void *, const uint8_t *, const void *, const void *, \
+                                       const uint8_t *, const void *, const void *, uint32_t, uint8_t *);
 #define PCGPU_INST_FR(C, EXT)                                                                                              \
   EXT template int fr_from_mont_impl<C>(pcgpu_ctx *, const void *, void *, size_t, uint32_t);                              \
   EXT template int fr_axpy_impl<C>(pcgpu_ctx *, void *, const void *, const void *, size_t, uint32_t);                     \

@@ -5,7 +5,7 @@
 // x 10 planes).  The callers with few terms -- the late rounds of the IPA
 // halving loop (ipa_pc/mod.rs:665-711), the verifier-side combinations (hyrax/mod.rs:498-504, kzg10/mod.rs:322-373), cfg1's
 // degree-2^10 commitments (kzg10/mod.rs:175-178) -- run here instead:
-//   grid  = (#problems) x W x split blocks, W = ceil((bits + 2) / c) windows of c = 6 bits; a window's terms are divided
+//   grid  = (#problems) x W x split blocks (the problems are a device array: the IPA's l and r, or Hyrax's 2 per checked proof), W = ceil((bits + 2) / c) windows of c = 6 bits; a window's terms are divided
 //           among `split` blocks (1 below 512 terms, else 3: 129 blocks, one wave on the 132 SMs of an H100), each producing a partial U_w
 //   block = 256 threads = 32 buckets (digit magnitudes 1..32) x 8 slices of the scalars
 //   1. digits: signed digits d in [-32, 31] by the offset trick: the base-2^c digits e_w of s + K, K = sum_w 2^(c-1) 2^(cw),
@@ -21,7 +21,7 @@
 
 namespace pcgpu {
 
-enum { SMALL_C = 6, SMALL_NB = 32, SMALL_SLICES = 8, SMALL_BLOCK = 256, SMALL_MAX_N = 4096, SMALL_MAX_PROB = 2, SMALL_SPLIT = 3, SMALL_SPLIT_MIN_N = 512 };
+enum { SMALL_C = 6, SMALL_NB = 32, SMALL_SLICES = 8, SMALL_BLOCK = 256, SMALL_MAX_N = 4096, SMALL_MAX_PROB = 1024, SMALL_SPLIT = 3, SMALL_SPLIT_MIN_N = 512 };
 
 template <class C>
 struct MsmSmallProblem {
@@ -48,7 +48,7 @@ PCGPU_DEV int small_digit(const uint32_t *s, const uint32_t *K, uint32_t w) {
 
 template <class C>
 struct MsmSmallBody {
-  MsmSmallProblem<C> prob[SMALL_MAX_PROB];
+  const MsmSmallProblem<C> *prob;   // device array, one entry per problem
   uint32_t mont;         // scalars are Montgomery Fr (converted in the digit pass) / canonical
   uint32_t split;        // blocks per window; block q of a window takes the terms i = q (mod split)
   XYZZ<C> *out;          // out[(p * W + w) * split + q] = partial U_w of problem p
